@@ -36,7 +36,7 @@ def load_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return json.load(open(p)), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return {"hbm_gbs": 6650.0}, "fallback 6.65 TB/s (B200_PROFILING.md)"
+    return {"hbm_gbs": 3350.0}, "fallback 3.35 TB/s (H100 SXM data sheet)"
 
 
 class ClockSampler(threading.Thread):
@@ -195,6 +195,36 @@ def run_reference(args):
     print(json.dumps(out))
 
 
+DUMP_LIMIT = 64 * 1024 * 1024
+
+
+def host_outputs(step_result):
+    """what one env.step() returned -- the observation dict, rewards, dones, info -- as float32 / float64 host arrays"""
+    import numpy as np
+
+    obs, rew, done, info = step_result
+    out = {k: v.float().cpu().numpy() for k, v in obs.items()}
+    out["reward"] = rew.float().cpu().numpy()
+    out["done"] = done.float().cpu().numpy()
+    out["info"] = info.cpu().numpy().astype(np.float64)  # int32 counters: exact in float64
+    return out
+
+
+def write_outputs(path, arrays):
+    """DIR/<name>.npy for every array; above DUMP_LIMIT bytes in all, the same seeded sample of env rows from each (row indices in env_index.npy)"""
+    import numpy as np
+
+    os.makedirs(path, exist_ok=True)
+    n = len(arrays["reward"])
+    total = sum(a.nbytes for a in arrays.values())
+    if total > DUMP_LIMIT:
+        keep = max(1, DUMP_LIMIT * n // (total + 8 * n))
+        rows = np.sort(np.random.RandomState(0).choice(n, keep, replace=False))
+        arrays = dict({k: a[rows] for k, a in arrays.items()}, env_index=rows.astype(np.float64))
+    for k, a in arrays.items():
+        np.save(os.path.join(path, k + ".npy"), a)
+
+
 def run_ours(args):
     import torch
 
@@ -265,7 +295,7 @@ def run_ours(args):
             a.zero_()
             a[:, -2:] = -1.0
     acts = [a.to(dev) for a in a_host]
-    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)  # > L2 (126 MB)
+    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)  # > L2 (50 MB on an H100)
 
     def barrier():
         if dist is not None:
@@ -284,10 +314,11 @@ def run_ours(args):
     for k in range(K):
         flush.fill_(float(k))  # evict L2 between timed iterations (not timed)
         ev[k][0].record()
-        env.step(acts[W + k])
+        last = env.step(acts[W + k])
         ev[k][1].record()
     barrier()
     clocks = sampler.stop()
+    dumped = host_outputs(last) if args.dump_outputs and rank == 0 else None
     step_ms = [a.elapsed_time(b) for a, b in ev]
     total_ms = torch.tensor([sum(step_ms)], device=dev, dtype=torch.float64)
     rank_ms = float(total_ms.item()) / K
@@ -369,8 +400,9 @@ def run_ours(args):
             if prof.get("build_id") == bid:
                 traffic = prof.get("dram_bytes_per_launch")
                 if prof.get("warp_instructions_per_launch") and clocks.get("sm_mhz"):
-                    slots = kernel_ms * 1e-3 * clocks["sm_mhz"] * 1e6 * 148 * 4  # warp-issue slots of the chip during one launch
-                    ipc = prof["warp_instructions_per_launch"] / (kernel_ms * 1e-3 * clocks["sm_mhz"] * 1e6 * 148)
+                    sms = torch.cuda.get_device_properties(dev).multi_processor_count
+                    slots = kernel_ms * 1e-3 * clocks["sm_mhz"] * 1e6 * sms * 4  # warp-issue slots of the chip during one launch
+                    ipc = prof["warp_instructions_per_launch"] / (kernel_ms * 1e-3 * clocks["sm_mhz"] * 1e6 * sms)
                     lanes = prof.get("lanes_active_per_instruction")
                     secondary = {"bound": "fp32-issue", "ipc": ipc, "ipc_peak": 4.0, "lanes_active": lanes,
                                  "frac": prof["warp_instructions_per_launch"] * lanes / 32.0 / slots,
@@ -404,6 +436,8 @@ def run_ours(args):
             v, n = cpu_env_rate(args.cpu_seconds)
             out["cpu_baseline"] = {"value": v, "unit": UNIT, "cores": 1, "kind": "port",
                                    "sample": "%d env.step() of one CPU oracle env (oracle/ref_env.py over oracle/fe_oracle.c) in %.0f s" % (n, args.cpu_seconds)}
+        if dumped is not None:
+            write_outputs(args.dump_outputs, dumped)
         print(json.dumps(out))
     if dist is not None:
         dist.barrier()
@@ -426,6 +460,8 @@ def main():
     ap.add_argument("--reward", default="sparse", choices=["sparse", "dense"], help="dense = FurnitureSawyerDenseRewardEnv (IKEASawyerDense-v0), one GPU, not the bench line")
     ap.add_argument("--ref-slice", type=float, default=1.0, help="--impl reference: seconds every worker runs free per bench step")
     ap.add_argument("--actions", default="random", choices=["random", "settled"])
+    ap.add_argument("--dump-outputs", metavar="DIR", help="after the timed steps, write what the last timed env.step() returned as DIR/<name>.npy "
+                    "(float32 / float64, at most 64 MB: a seeded sample of env rows above that)")
     args = ap.parse_args()
     if args.warmup < 3:
         args.warmup = 3

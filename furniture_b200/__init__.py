@@ -1,2 +1,2 @@
-"""furniture_b200: B200-native batched physics backend for the furniture-assembly env hot path."""
+"""furniture_b200: H100-native (sm_90a) batched physics backend for the furniture-assembly env hot path."""
 __version__ = "0.1.0"

@@ -4,7 +4,7 @@
 #include "fe_engine.h"
 
 #define FE_MAX_WPB 14      /* warps (= envs) per block of the sim / step / reset kernels */
-#define FE_EXTRA_BLOCKS 148 /* spare blocks of the step grid: heavy envs get half-empty blocks */
+#define FE_EXTRA_BLOCKS 132 /* spare blocks of the step grid, one per SM of an H100 SXM: heavy envs get half-empty blocks */
 
 struct FeState {
   int N;

@@ -1,6 +1,6 @@
 // fe_engine.h -- one mj_step for one environment, executed by one warp out of its shared-memory slice.
 //
-// This is the B200-native replacement of the per-env MjSim.step() hot loop (reference call site
+// This is the GPU-native replacement of the per-env MjSim.step() hot loop (reference call site
 // furniture/env/furniture.py:2878-2879; the arithmetic is MuJoCo's mj_step, see DESIGN.md for the stage map):
 //   fe_kin_smooth : forward kinematics over the fused link tree, link velocities, composite inertia (CRBA) of the
 //                   robot block, spatial inertia of every free part, RNE bias wrench, actuation, qacc_smooth

@@ -170,7 +170,7 @@ static int plat_module(fe_handle* h) {
   FeModule* m = new FeModule();
   m->device = h->device; m->lay = h->lay; m->users = 1;
   CUresult r = g_drv.ModuleLoadData(&m->mod, fe_cubin_start);
-  if (r != CUDA_SUCCESS) { delete m; return fail(h, -10, "cuModuleLoadData(embedded sm_100a cubin): " + drv_err(r) + " (this library runs on B200 / sm_100a only)"); }
+  if (r != CUDA_SUCCESS) { delete m; return fail(h, -10, "cuModuleLoadData(embedded sm_90a cubin): " + drv_err(r) + " (this library runs on H100 / sm_90a only)"); }
   struct { const char* name; CUfunction* f; } fn[] = {{"fe_sim_kernel", &m->f_sim}, {"fe_env_step_kernel", &m->f_step}, {"fe_env_reset_kernel", &m->f_reset},
                                                       {"fe_order_kernel", &m->f_order}, {"fe_is_aligned_kernel", &m->f_aligned}, {"fe_dense_eval_kernel", &m->f_dense}};
   for (auto& f : fn) {

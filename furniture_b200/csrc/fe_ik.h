@@ -10,8 +10,8 @@
 //                         the same algorithm in float64 (oracle/ik_oracle.py)
 // The part of an env step that follows the simulation (connect, reward, termination, observation) is the one of fe_env.h:
 // fe_ik_controls / fe_ik_finish below restate fe_env_step_one's blocks with the policy action (8 numbers) and the low-level action
-// (7 velocities + gripper) as separate arguments.  fe_env.h itself is left untouched on purpose: its step kernel is the build the
-// committed ncu capture belongs to (profiles/traffic.json); fold the two once the next capture is taken.
+// (7 velocities + gripper) as separate arguments.  fe_env.h itself is left untouched on purpose: its step kernel is the stock build
+// that is profiled and benched (profiles/); fold the two once a capture of the folded build is taken.
 #pragma once
 #include "fe_env.h"
 

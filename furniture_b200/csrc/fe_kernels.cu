@@ -1,4 +1,4 @@
-// fe_kernels.cu -- the sm_100a kernels, compiled to a cubin (nvcc -cubin) that the host library embeds and loads through
+// fe_kernels.cu -- the sm_90a kernels, compiled to a cubin (nvcc -cubin) that the host library embeds and loads through
 // the driver API: one module instance per (device, slice layout).  The slice layout table `fe_c_lay` is a __constant__
 // object of the module, so every instance carries its own copy and handles of different models (a mixed-furniture batch)
 // run concurrently on their own streams without re-uploading it.

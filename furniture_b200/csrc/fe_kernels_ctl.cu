@@ -1,5 +1,5 @@
 // fe_kernels_ctl.cu -- the step kernel of the torque controllers (fe_ctl.h) and the test hook of their arithmetic, compiled to their own
-// sm_100a cubin (like fe_kernels_ik.cu: the stock kernels stay the profiled binary).  Same launch shape as fe_env_step_kernel.
+// sm_90a cubin (like fe_kernels_ik.cu: the stock kernels stay the profiled binary).  Same launch shape as fe_env_step_kernel.
 #include <stdint.h>
 
 #include "../../include/furniture_b200.h"

@@ -1,4 +1,4 @@
-// fe_kernels_ik.cu -- the step kernel of control_type="ik" (fe_ik.h), compiled to its own sm_100a cubin: the stock kernels of
+// fe_kernels_ik.cu -- the step kernel of control_type="ik" (fe_ik.h), compiled to its own sm_90a cubin: the stock kernels of
 // fe_kernels.cu stay the binary they were profiled as.  Same launch shape as fe_env_step_kernel: one warp = one env, envs packed into
 // blocks by fe_order_kernel.
 #include <stdint.h>

@@ -3,7 +3,7 @@
 // Every physics routine is written as a sequence of *lane regions*: inside LANES_BEGIN/LANES_END each of the 32
 // lanes runs the body with its own `lane`; lanes talk to each other only through the warp's shared-memory slice and
 // only across a region boundary (LANES_END is a __syncwarp()).  Reductions / ballots are done between regions on a
-// scratch array.  On sm_100a this compiles to straight SIMT code (the lane loop has one trip).  The same source also
+// scratch array.  On sm_90a this compiles to straight SIMT code (the lane loop has one trip).  The same source also
 // builds with a host compiler (FE_EMULATE) where a region is a 32-trip loop -- used ONLY by the CPU test harness
 // (tests/emu) so kernel logic can be exercised without a GPU; the product never loads that build.
 #pragma once

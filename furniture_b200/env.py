@@ -352,7 +352,7 @@ class MixedFurnitureEnv:
 
 def model_costs():
     """measured GPU time per env-step per env (microseconds) of every compiled Sawyer scene: compiled/cost.json, written by
-    tools/calibrate_models.py on a B200; {} when absent"""
+    tools/calibrate_models.py on an H100; {} when absent"""
     import json
     import os
 

@@ -1,4 +1,4 @@
-/* furniture_b200.h -- C-ABI of the B200-native batched physics backend.
+/* furniture_b200.h -- C-ABI of the H100-native (sm_90a) batched physics backend.
  *
  * The reference has no FFI seam of its own: FurnitureEnv drives the closed MuJoCo 2.0 binary through mujoco-py
  * (SURVEY.md 8b-B2).  This header is the seam a maintainer would bind instead; every entry point names the

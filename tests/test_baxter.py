@@ -1,6 +1,6 @@
 """FurnitureBaxterEnv (BASELINE.json config 4: Baxter + chair_ingolf_0650; furniture/env/furniture_baxter.py): two arms, 17
 actions, 58 + 35 observations, per-arm finger scans, armature / margin / capsule / <exclude> in the model.  The device env is
-compared with the CPU env oracle (oracle/ref_env.py) from the same seeds: `emu` = lane-emulated build, `cuda` = the sm_100a library."""
+compared with the CPU env oracle (oracle/ref_env.py) from the same seeds: `emu` = lane-emulated build, `cuda` = the sm_90a library."""
 import numpy as np
 import pytest
 

@@ -68,7 +68,7 @@ def test_engine_refuses_to_run_without_the_cuda_library(tmp_path):
 
 @pytest.mark.parametrize("gpu", [pytest.param(False, id="emu"), pytest.param(True, id="cuda", marks=pytest.mark.gpu)])
 def test_get_and_set_state_round_trip(gpu):
-    """fe_get_state / fe_set_state (get_env_state / set_env_state, furniture.py:1781-1803) on the lane-emulated build and on the sm_100a library:
+    """fe_get_state / fe_set_state (get_env_state / set_env_state, furniture.py:1781-1803) on the lane-emulated build and on the sm_90a library:
     the state planted comes back bit for bit, and stepping from it equals stepping from the same state planted field by field"""
     import sys
 

@@ -1,6 +1,6 @@
 """A binder without Python: examples/step_from_c.c is compiled against include/furniture_b200.h and libfurniture_b200.so, creates its handle
 from a compiled scene file (fe_create_from_file) and steps it with host buffers.  Without a GPU the program must end with the library's
-error message and exit code 2 (no crash, no CPU fallback); on the B200 it steps."""
+error message and exit code 2 (no crash, no CPU fallback); on an H100 it steps."""
 import os
 import subprocess
 

@@ -1,6 +1,6 @@
 """FurnitureCursorEnv (BASELINE.json config 1: Cursor + toy_table, one env; furniture/env/furniture_cursor.py + the Cursor
 branches of furniture.py).  The host logic of furniture_b200/cursor_env.py is run twice from the same seed and actions: over the
-engine (lane-emulated build here, the sm_100a library when marked gpu) and over the fp64 CPU oracle through the same backend
+engine (lane-emulated build here, the sm_90a library when marked gpu) and over the fp64 CPU oracle through the same backend
 interface.  Decisions (selection, rollbacks, connect steps, welds) must be identical, poses equal to fp32 tolerance."""
 import numpy as np
 import pytest

@@ -1,7 +1,7 @@
 """Parity of the engine kernels against the CPU oracle (oracle/fe_oracle.c) on the same seeded inputs.
 
 Each test runs twice: `emu` = the lane-emulated harness build of the kernel source (CPU, keeps the kernel logic covered
-when no GPU is present) and `cuda` = the real sm_100a library through the C-ABI (marked gpu).  Tolerances are fp32-vs-fp64
+when no GPU is present) and `cuda` = the real sm_90a library through the C-ABI (marked gpu).  Tolerances are fp32-vs-fp64
 and written next to each assertion.  Reference path being replaced: MjSim.forward()/step(), furniture.py:2877-2879."""
 import os
 

@@ -1,6 +1,6 @@
 """Env-level parity: the device FurnitureEnv logic (fe_env_step / fe_env_reset through the C-ABI) against the CPU
 env oracle (oracle/ref_env.py, a restatement of FurnitureSawyerEnv with control_type="impedance").
-`emu` runs the lane-emulated harness build on CPU, `cuda` the sm_100a library (marked gpu)."""
+`emu` runs the lane-emulated harness build on CPU, `cuda` the sm_90a library (marked gpu)."""
 import json
 import os
 
@@ -419,7 +419,7 @@ def test_single_step_parity_along_a_drifting_rollout(gpu):
 def test_connect_decisions_over_perturbed_alignments(gpu):
     """48 variations of the grasp-and-align state: the table top displaced (up to a few cm) and rotated (up to 25 degrees) away from
     the aligned pose, so that some requests connect and others must not.  Every decision (num_connected, weld activation), reward and
-    post-connect state of the device env equals the CPU env's (lane-emulated build and, gpu-marked, the sm_100a library)."""
+    post-connect state of the device env equals the CPU env's (lane-emulated build and, gpu-marked, the sm_90a library)."""
     m = mjcf.load_scene("Sawyer", "table_lack_0825")
     env0 = OracleFurnitureEnv(m)
     env0.reset()

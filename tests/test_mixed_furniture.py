@@ -3,7 +3,7 @@ tree (64 models; 3 of them with mesh colliders, which collide through their conv
 parts, 1 to 37 welds, boxes, cylinders and hulls.  For each model: device reset (settle protocol of furniture.py:1406-1663), then
 env steps with random actions compared with the CPU env oracle started from the same post-reset state.
 
-`emu` = lane-emulated harness build of the kernel source (CPU); `cuda` = the sm_100a library (marked gpu, a subset that
+`emu` = lane-emulated harness build of the kernel source (CPU); `cuda` = the sm_90a library (marked gpu, a subset that
 spans the shapes: most parts, most geoms, cylinders, smallest)."""
 import glob
 import os

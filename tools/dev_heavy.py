@@ -15,7 +15,7 @@ from parity_util import settled_state
 qs = settled_state(m, 0, dz=0.0)
 q2 = qs.copy(); q2[:9] = q[:9]; q2[9:16] = q[9:16]  # leg 0 between the pads; the other parts rest on the floor
 q = q2
-for N in [int(a) for a in sys.argv[1:]] or [1, 7, 148 * 7, 4096]:
+for N in [int(a) for a in sys.argv[1:]] or [1, 7, 132 * 7, 4096]:
     eng = Engine(m, N, 0, default_config(), lib_path=os.environ.get("FE_LIB"))
     eng.env_reset()
     eng.set("qpos", q); eng.set("qvel", np.zeros(m.nv)); eng.set("qacc_warmstart", np.zeros(m.nv)); eng.forward()
