@@ -9,6 +9,7 @@
 // Kept quirks: the ramp is ramp_steps = floor(0.2 * control_freq / timestep) = 2000 mj_steps long; the position controller fixes its
 // orientation goal once per controller lifetime (ori_set survives resets).
 #pragma once
+#include "fe_env.h"
 
 enum { FE_CTL_JOINT_TORQUE = 0, FE_CTL_JOINT_VELOCITY = 1, FE_CTL_JOINT_IMPEDANCE = 2, FE_CTL_POS_ORI = 3, FE_CTL_POS = 4 };
 
@@ -184,8 +185,6 @@ FE_HDN void fe_ctl_eval_episode(const fe_ctl_config* c, int first, int count, co
 }
 
 // ---------------------------------------------------------------- the env step under a torque controller
-// (needs FeEnv of fe_env.h and fe_ik_finish of fe_ik.h: include those first; host builds that only want the arithmetic above need not)
-#ifdef FE_SCENE_MAGIC
 struct FeCtlArgs {
   const fe_ctl_config* c;
   FeCtlState* st;
@@ -239,7 +238,7 @@ FE_FN void fe_env_ctl_step_one(FeEnv* e, FeCtlArgs ctl, const float* action, flo
   LANES_BEGIN
     if (lane == 0) {
       if (e->es.episode_len[e->env] == 0) fe_ctl_reset(c, st); // _reset: controller.reset() (furniture.py:1885-1887)
-      e->ei[0] = 0; e->ei[1] = -1; e->ei[6] = 0; w->u()[2] = 0;
+      fe_env_clear_flags(e);
     }
   LANES_END
   fe_forward(w); // sim.forward() ahead of the loop (:3080): the first _pre_action reads fresh kinematics
@@ -262,6 +261,5 @@ FE_FN void fe_env_ctl_step_one(FeEnv* e, FeCtlArgs ctl, const float* action, flo
     fe_substep_lockstep(w);
   }
   const int fail = (w->u()[2] & 8) ? 1 : 0;
-  fe_ik_finish(e, a, act_dim, connect, fail, fail, reward_out, done_out, info_out);
+  fe_env_finish(e, a, act_dim, connect, fail, fail, reward_out, done_out, info_out);
 }
-#endif

@@ -3,7 +3,8 @@
 //   fe_env_step_one  : FurnitureEnv.step -> FurnitureSawyerEnv._step -> _step_continuous (action mapping, gravity
 //                      compensation, nsub mj_steps, finger-contact scan, _try_connect/_is_aligned/_connect), post-connect
 //                      re-pin, _get_obs, _compute_reward, _after_step, VecEnv auto-reset
-//                      (furniture/env/furniture.py:364-480, :1260-1330, :3332-3379; furniture_sawyer.py:66-155)
+//                      (furniture/env/furniture.py:364-480, :1260-1330, :3332-3379; furniture_sawyer.py:66-155); its parts before and
+//                      after the simulation, fe_env_controls / fe_env_finish, are also those of the IK and torque-controller steps
 //   fe_env_reset_one : FurnitureEnv._reset settle protocol (furniture.py:1406-1663) with a counter-based per-env RNG
 //   fe_is_aligned_d  : _is_aligned in float64 with numpy's exact arithmetic (float32 unit_vector, FMA-chain dots)
 #pragma once
@@ -598,17 +599,15 @@ FE_FN void fe_env_reset_one(FeEnv* e) {
   fe_write_obs(e);
 }
 
-// FurnitureEnv.step for one env; writes reward / done / info; auto-resets when done (subproc_vec_env.py:16-20)
-FE_FN void fe_env_step_one(FeEnv* e, const float* action, float* reward_out, uint8_t* done_out, int32_t* info_out) {
+// the per-step flags: no connection found, no re-pin pending, no auto-reset due, no simulation failure yet (lane 0)
+FE_HD void fe_env_clear_flags(FeEnv* e) { e->ei[0] = 0; e->ei[1] = -1; e->ei[6] = 0; e->w->u()[2] = 0; }
+
+// _setup_action + gravity compensation with the low-level action `a` (indexed by act_src) and the gripper action `grip`
+FE_HD void fe_env_controls(FeEnv* e, const float* a, float grip) {
   FeWarp* w = e->w;
   const fe_model* m = w->m;
   const fe_scene* sc = e->sc;
   const fe_config* cfg = e->cfg;
-  const int nr = m->nr, np = m->npart, env = e->env;
-  const float* a = action + (size_t)env * sc->act_dim;
-  float grip = sc->grip_action_index >= 0 ? a[sc->grip_action_index] : 0.f;
-  if (cfg->discrete_grip) grip = grip < 0.f ? -1.f : 1.f; // FurnitureSawyerEnv._step only (furniture_sawyer.py:73-74); Baxter: index -1
-  const float connect = a[sc->connect_action_index];
   LANES_BEGIN
     for (int u = lane; u < m->nu; u += 32) { // _setup_action, furniture.py:3332-3367
       const int src = sc->act_src[u];
@@ -623,12 +622,20 @@ FE_FN void fe_env_step_one(FeEnv* e, const float* action, float* reward_out, uin
     }
     for (int i = lane; i < sc->narm; i += 32) w->qfrc_applied()[sc->arm_dof[i]] = w->bias()[sc->arm_dof[i]]; // gravity compensation, :3372-3377
     for (int i = lane; i < sc->ngrip; i += 32) w->qfrc_applied()[sc->grip_dof[i]] = w->bias()[sc->grip_dof[i]];
-    if (lane == 0) { e->ei[0] = 0; e->ei[1] = -1; e->ei[6] = 0; w->u()[2] = 0; }
+    if (lane == 0) fe_env_clear_flags(e);
   LANES_END
-  for (int i = 0; i < cfg->nsub; ++i) fe_substep_lockstep(w); // _do_simulation, furniture.py:2877-2879
-  int fail = (w->u()[2] & 8) ? 1 : 0;                   // MujocoException path, :2889-2897
+}
+
+// what follows the simulation in FurnitureEnv.step, with the policy action `a` (act_dim numbers) for reward and connect
+// `fail`: some _do_simulation of this step raised; `reset_now`: the last one did, so the env has not been reset for it yet
+FE_HD void fe_env_finish(FeEnv* e, const float* a, int act_dim, float connect, int fail, int reset_now, float* reward_out, uint8_t* done_out, int32_t* info_out) {
+  FeWarp* w = e->w;
+  const fe_model* m = w->m;
+  const fe_scene* sc = e->sc;
+  const fe_config* cfg = e->cfg;
+  const int np = m->npart, env = e->env;
   FE_SYNC;
-  if (fail) {
+  if (reset_now) {
     fe_env_reset_one(e);
   } else {
     if (connect > 0.f) { // furniture.py:1290-1322: per arm, the first part both of its fingers touch; stop at the first connection
@@ -677,7 +684,7 @@ FE_FN void fe_env_step_one(FeEnv* e, const float* action, float* reward_out, uin
       const int connected_now = nc != e->es.prev_num_connected[env]; // _connected: a connection was made during this step
       e->es.prev_num_connected[env] = nc;
       float sq = 0.f;
-      for (int k = 0; k < sc->act_dim; ++k) sq += a[k] * a[k];
+      for (int k = 0; k < act_dim; ++k) sq += a[k] * a[k];
       float reward = success_r + touch_r + pick_r - cfg->ctrl_penalty_coef * sq;
       int success = (nc == np - 1 && np > 1) ? 1 : 0;
       int done = success;
@@ -685,10 +692,10 @@ FE_FN void fe_env_step_one(FeEnv* e, const float* action, float* reward_out, uin
         FeSliceWorld world = {w};
         const double thr[4] = {cfg->alignment_pos_dist, cfg->alignment_rot_dist_up, cfg->alignment_rot_dist_forward, cfg->alignment_project_dist};
         double ad[FE_MAXU + 2], dr = 0.0, di[FE_DENSE_INFO];
-        for (int k = 0; k < sc->act_dim; ++k) ad[k] = (double)a[k];
+        for (int k = 0; k < act_dim; ++k) ad[k] = (double)a[k];
         int dd = 0;
         FeDenseState* ds = e->es.dstate + env;
-        fe_dense_step(world, e->es.dense, &sc->dense, thr, np - 1, ds, ad, sc->act_dim, connected_now, &dr, &dd, di);
+        fe_dense_step(world, e->es.dense, &sc->dense, thr, np - 1, ds, ad, act_dim, connected_now, &dr, &dd, di);
         reward = (float)dr;
         success = ds->success;
         done = done || dd;
@@ -715,6 +722,21 @@ FE_FN void fe_env_step_one(FeEnv* e, const float* action, float* reward_out, uin
   if (e->ei[6]) fe_env_reset_one(e); else fe_write_obs(e);
 }
 
+// FurnitureEnv.step for one env; writes reward / done / info; auto-resets when done (subproc_vec_env.py:16-20)
+FE_FN void fe_env_step_one(FeEnv* e, const float* action, float* reward_out, uint8_t* done_out, int32_t* info_out) {
+  FeWarp* w = e->w;
+  const fe_scene* sc = e->sc;
+  const fe_config* cfg = e->cfg;
+  const float* a = action + (size_t)e->env * sc->act_dim;
+  float grip = sc->grip_action_index >= 0 ? a[sc->grip_action_index] : 0.f;
+  if (cfg->discrete_grip) grip = grip < 0.f ? -1.f : 1.f; // FurnitureSawyerEnv._step only (furniture_sawyer.py:73-74); Baxter: index -1
+  const float connect = a[sc->connect_action_index];
+  fe_env_controls(e, a, grip);
+  for (int i = 0; i < cfg->nsub; ++i) fe_substep_lockstep(w); // _do_simulation, furniture.py:2877-2879
+  const int fail = (w->u()[2] & 8) ? 1 : 0;             // MujocoException path, :2889-2897
+  fe_env_finish(e, a, sc->act_dim, connect, fail, fail, reward_out, done_out, info_out);
+}
+
 // per-env context set-up shared by the CUDA kernels and the emulation loop
 FE_FN void fe_env_bind(FeEnv* e, float* slice, const fe_model* m, const fe_scene* sc, const fe_config* cfg, const FeOpt& opt, const FeState& st,
                        const FeEnvState& es, int env, int slice_words_physics) {
@@ -733,4 +755,16 @@ FE_FN void fe_env_load_groups(FeEnv* e) {
 FE_FN void fe_env_store_groups(FeEnv* e) {
   const int np = e->w->m->npart;
   LANES_BEGIN for (int p = lane; p < np; p += 32) e->es.group[(size_t)e->env * np + p] = e->group[p]; LANES_END
+}
+// one env in its slice: bind, load the env's state from HBM, run `body(FeEnv*)` (a reset or a step), store the state back
+template <class Body>
+FE_HD void fe_env_run(float* slice, const fe_model* m, const fe_scene* sc, const fe_config* cfg, const FeOpt& opt, const FeState& st, const FeEnvState& es,
+                      int env, int slice_words_physics, Body body) {
+  FeEnv e;
+  fe_env_bind(&e, slice, m, sc, cfg, opt, st, es, env, slice_words_physics);
+  fe_load(e.w, st, env);
+  fe_env_load_groups(&e);
+  body(&e);
+  fe_env_store_groups(&e);
+  fe_store(e.w, st, env);
 }

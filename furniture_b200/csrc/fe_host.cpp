@@ -49,12 +49,6 @@ static int plat_ctl_eval(fe_handle* h, const struct fe_ctl_config* cc, int n_epi
 // ---------------------------------------------------------------- embedded cubin + driver entry points
 __asm__(".section .rodata\n.balign 16\n.global fe_cubin_start\nfe_cubin_start:\n.incbin \"" FE_CUBIN_FILE "\"\n.global fe_cubin_end\nfe_cubin_end:\n.byte 0\n.previous\n");
 extern "C" const unsigned char fe_cubin_start[];
-// the IK step kernel is a module of its own (fe_kernels_ik.cu): the stock kernels stay the binary they were profiled as
-__asm__(".section .rodata\n.balign 16\n.global fe_cubin_ik_start\nfe_cubin_ik_start:\n.incbin \"" FE_CUBIN_IK_FILE "\"\n.global fe_cubin_ik_end\nfe_cubin_ik_end:\n.byte 0\n.previous\n");
-extern "C" const unsigned char fe_cubin_ik_start[];
-// likewise the torque controllers (fe_kernels_ctl.cu)
-__asm__(".section .rodata\n.balign 16\n.global fe_cubin_ctl_start\nfe_cubin_ctl_start:\n.incbin \"" FE_CUBIN_CTL_FILE "\"\n.global fe_cubin_ctl_end\nfe_cubin_ctl_end:\n.byte 0\n.previous\n");
-extern "C" const unsigned char fe_cubin_ctl_start[];
 
 struct DriverApi {
   CUresult (*ModuleLoadData)(CUmodule*, const void*) = nullptr;
@@ -98,11 +92,7 @@ struct FeModule {
   int device;
   FeLayout lay;
   CUmodule mod;
-  CUfunction f_sim, f_step, f_reset, f_order, f_aligned, f_dense;
-  CUmodule mod_ik = nullptr;     // loaded when a handle of this (device, layout) first steps with control_type="ik"
-  CUfunction f_ik_step = nullptr;
-  CUmodule mod_ctl = nullptr;    // the torque controllers' module, loaded on first use
-  CUfunction f_ctl_step = nullptr, f_ctl_eval = nullptr;
+  CUfunction f_sim, f_step, f_ik_step, f_ctl_step, f_reset, f_order, f_aligned, f_dense, f_ctl_eval;
   int users;
 };
 static std::vector<FeModule*> g_modules;
@@ -137,18 +127,13 @@ static int plat_enter(fe_handle* h) {
 static void plat_leave(fe_handle* h, int prev) {
   if (prev >= 0 && prev != h->device) cudaSetDevice(prev);
 }
-struct DevScope {
-  fe_handle* h; int prev;
-  explicit DevScope(fe_handle* h_) : h(h_), prev(plat_enter(h_)) {}
-  ~DevScope() { plat_leave(h, prev); }
-};
 
 static int plat_init(fe_handle* h) {
   int ndev = 0;
   cudaError_t e = cudaGetDeviceCount(&ndev);
   if (e != cudaSuccess) { h->err = std::string("cudaGetDeviceCount: ") + cudaGetErrorString(e); return -10; }
   if (h->device < 0 || h->device >= ndev) { h->err = "fe_create: no such CUDA device"; return -10; }
-  DevScope dev(h);
+  FeDevScope dev(h);
   cudaFree(0); // make sure the primary context of the device exists and is current
   CudaPlat* p = new CudaPlat();
   h->plat = p;
@@ -171,8 +156,10 @@ static int plat_module(fe_handle* h) {
   m->device = h->device; m->lay = h->lay; m->users = 1;
   CUresult r = g_drv.ModuleLoadData(&m->mod, fe_cubin_start);
   if (r != CUDA_SUCCESS) { delete m; return fail(h, -10, "cuModuleLoadData(embedded sm_90a cubin): " + drv_err(r) + " (this library runs on H100 / sm_90a only)"); }
-  struct { const char* name; CUfunction* f; } fn[] = {{"fe_sim_kernel", &m->f_sim}, {"fe_env_step_kernel", &m->f_step}, {"fe_env_reset_kernel", &m->f_reset},
-                                                      {"fe_order_kernel", &m->f_order}, {"fe_is_aligned_kernel", &m->f_aligned}, {"fe_dense_eval_kernel", &m->f_dense}};
+  struct { const char* name; CUfunction* f; } fn[] = {
+      {"fe_sim_kernel", &m->f_sim}, {"fe_env_step_kernel", &m->f_step}, {"fe_env_ik_step_kernel", &m->f_ik_step}, {"fe_env_ctl_step_kernel", &m->f_ctl_step},
+      {"fe_env_reset_kernel", &m->f_reset}, {"fe_order_kernel", &m->f_order}, {"fe_is_aligned_kernel", &m->f_aligned}, {"fe_dense_eval_kernel", &m->f_dense},
+      {"fe_ctl_eval_kernel", &m->f_ctl_eval}};
   for (auto& f : fn) {
     r = g_drv.ModuleGetFunction(f.f, m->mod, f.name);
     if (r != CUDA_SUCCESS) { g_drv.ModuleUnload(m->mod); delete m; return fail(h, -10, std::string("cuModuleGetFunction ") + f.name + ": " + drv_err(r)); }
@@ -182,8 +169,8 @@ static int plat_module(fe_handle* h) {
   r = g_drv.ModuleGetGlobal(&sym, &bytes, m->mod, "fe_c_lay");
   if (r == CUDA_SUCCESS && bytes != sizeof(FeLayout)) r = CUDA_ERROR_INVALID_VALUE;
   if (r == CUDA_SUCCESS) r = g_drv.MemcpyHtoD(sym, &h->lay, sizeof(FeLayout));
-  // the opt-in shared-memory limit is an attribute of the function: always the hardware maximum (227 KB)
-  for (CUfunction f : {m->f_sim, m->f_step, m->f_reset})
+  // the opt-in shared-memory limit is an attribute of the function: always the hardware maximum (227 KB), for the kernels that run in slices
+  for (CUfunction f : {m->f_sim, m->f_step, m->f_ik_step, m->f_ctl_step, m->f_reset})
     if (r == CUDA_SUCCESS) r = g_drv.FuncSetAttribute(f, CU_FUNC_ATTRIBUTE_MAX_DYNAMIC_SHARED_SIZE_BYTES, 227 * 1024);
   if (r != CUDA_SUCCESS) { g_drv.ModuleUnload(m->mod); delete m; return fail(h, -10, "module set-up (fe_c_lay / shared-memory limit): " + drv_err(r)); }
   g_modules.push_back(m);
@@ -227,7 +214,7 @@ static int plat_prepare(fe_handle* h) {
 static void plat_fini(fe_handle* h) {
   CudaPlat* p = (CudaPlat*)h->plat;
   if (!p) return;
-  DevScope dev(h);
+  FeDevScope dev(h);
   cudaDeviceSynchronize();
   if (p->pin_act) cudaFreeHost(p->pin_act);
   if (p->pin_out) cudaFreeHost(p->pin_out);
@@ -241,17 +228,15 @@ static void plat_fini(fe_handle* h) {
       for (size_t i = 0; i < g_modules.size(); ++i)
         if (g_modules[i] == p->km) { g_modules.erase(g_modules.begin() + i); break; }
       g_drv.ModuleUnload(p->km->mod);
-      if (p->km->mod_ik) g_drv.ModuleUnload(p->km->mod_ik);
-      if (p->km->mod_ctl) g_drv.ModuleUnload(p->km->mod_ctl);
       delete p->km;
     }
   }
   delete p;
   h->plat = nullptr;
 }
-static void plat_sync(fe_handle* h) { DevScope dev(h); cudaDeviceSynchronize(); }
+static void plat_sync(fe_handle* h) { FeDevScope dev(h); cudaDeviceSynchronize(); }
 static void plat_copy_d2d(fe_handle* h, void* dst, const void* src, size_t n, void* stream) {
-  DevScope dev(h);
+  FeDevScope dev(h);
   if (dst != src) cudaMemcpyAsync(dst, src, n, cudaMemcpyDeviceToDevice, (cudaStream_t)stream);
 }
 static void note_stream(CudaPlat* p, cudaStream_t s) { p->last_stream = s; p->any_launch = true; }
@@ -260,64 +245,18 @@ static int launch(fe_handle* h, CUfunction f, unsigned grid, unsigned block, siz
   DRV_OK(g_drv.LaunchKernel(f, grid, 1, 1, block, 1, 1, (unsigned)smem, (CUstream)stream, args, nullptr));
   return 0;
 }
-// the IK module of this handle's (device, layout): its own copy of the slice layout table
-static int plat_module_ik(fe_handle* h) {
-  CudaPlat* p = (CudaPlat*)h->plat;
-  std::lock_guard<std::mutex> lock(g_mu);
-  FeModule* m = p->km;
-  if (m->f_ik_step) return 0;
-  CUmodule mod = nullptr;
-  CUfunction f = nullptr;
-  CUresult r = g_drv.ModuleLoadData(&mod, fe_cubin_ik_start);
-  if (r != CUDA_SUCCESS) return fail(h, -10, "cuModuleLoadData(embedded IK cubin): " + drv_err(r));
-  r = g_drv.ModuleGetFunction(&f, mod, "fe_env_ik_step_kernel");
-  CUdeviceptr sym = 0;
-  size_t bytes = 0;
-  if (r == CUDA_SUCCESS) r = g_drv.ModuleGetGlobal(&sym, &bytes, mod, "fe_c_lay");
-  if (r == CUDA_SUCCESS && bytes != sizeof(FeLayout)) r = CUDA_ERROR_INVALID_VALUE;
-  if (r == CUDA_SUCCESS) r = g_drv.MemcpyHtoD(sym, &h->lay, sizeof(FeLayout));
-  if (r == CUDA_SUCCESS) r = g_drv.FuncSetAttribute(f, CU_FUNC_ATTRIBUTE_MAX_DYNAMIC_SHARED_SIZE_BYTES, 227 * 1024);
-  if (r != CUDA_SUCCESS) { g_drv.ModuleUnload(mod); return fail(h, -10, "IK module set-up: " + drv_err(r)); }
-  m->mod_ik = mod; m->f_ik_step = f;
-  return 0;
-}
-static int plat_module_ctl(fe_handle* h) {
-  CudaPlat* p = (CudaPlat*)h->plat;
-  std::lock_guard<std::mutex> lock(g_mu);
-  FeModule* m = p->km;
-  if (m->f_ctl_step) return 0;
-  CUmodule mod = nullptr;
-  CUfunction f = nullptr, fe = nullptr;
-  CUresult r = g_drv.ModuleLoadData(&mod, fe_cubin_ctl_start);
-  if (r != CUDA_SUCCESS) return fail(h, -10, "cuModuleLoadData(embedded controller cubin): " + drv_err(r));
-  r = g_drv.ModuleGetFunction(&f, mod, "fe_env_ctl_step_kernel");
-  if (r == CUDA_SUCCESS) r = g_drv.ModuleGetFunction(&fe, mod, "fe_ctl_eval_kernel");
-  CUdeviceptr sym = 0;
-  size_t bytes = 0;
-  if (r == CUDA_SUCCESS) r = g_drv.ModuleGetGlobal(&sym, &bytes, mod, "fe_c_lay");
-  if (r == CUDA_SUCCESS && bytes != sizeof(FeLayout)) r = CUDA_ERROR_INVALID_VALUE;
-  if (r == CUDA_SUCCESS) r = g_drv.MemcpyHtoD(sym, &h->lay, sizeof(FeLayout));
-  if (r == CUDA_SUCCESS) r = g_drv.FuncSetAttribute(f, CU_FUNC_ATTRIBUTE_MAX_DYNAMIC_SHARED_SIZE_BYTES, 227 * 1024);
-  if (r != CUDA_SUCCESS) { g_drv.ModuleUnload(mod); return fail(h, -10, "controller module set-up: " + drv_err(r)); }
-  m->mod_ctl = mod; m->f_ctl_step = f; m->f_ctl_eval = fe;
-  return 0;
-}
 static int launch_step(fe_handle* h, const float* actions, float* reward, uint8_t* done, int32_t* info, cudaStream_t stream) {
   CudaPlat* p = (CudaPlat*)h->plat;
   int slice_words = h->slice_words;
   const int* slots = p->slots;
-  if (h->ctl.c) { // one of the NEW_CONTROLLERS: same launch shape, the kernel of the controllers' module
-    if (int rc = plat_module_ctl(h)) return rc;
-    void* a[] = {&h->st, &h->es, &h->ctl, &h->dm, &h->ds, &h->cfg, &h->opt, &actions, &reward, &done, &info, &slice_words, &slots};
-    if (int rc = launch(h, p->km->f_ctl_step, p->nblocks, 32 * p->wpb, p->smem_env, stream, a)) return rc;
-  } else if (h->ik.c) { // control_type="ik": same launch shape, the IK kernel of the second module
-    if (int rc = plat_module_ik(h)) return rc;
-    void* a[] = {&h->st, &h->es, &h->ik, &h->dm, &h->ds, &h->cfg, &h->opt, &actions, &reward, &done, &info, &slice_words, &slots};
-    if (int rc = launch(h, p->km->f_ik_step, p->nblocks, 32 * p->wpb, p->smem_env, stream, a)) return rc;
-  } else {
-  void* a[] = {&h->st, &h->es, &h->dm, &h->ds, &h->cfg, &h->opt, &actions, &reward, &done, &info, &slice_words, &slots};
-  if (int rc = launch(h, p->km->f_step, p->nblocks, 32 * p->wpb, p->smem_env, stream, a)) return rc;
-  }
+  // the IK and torque-controller step kernels take their control arguments right after es; all three have the same launch shape
+  CUfunction f = p->km->f_step;
+  void* control = nullptr;
+  if (h->ctl.c) { f = p->km->f_ctl_step; control = &h->ctl; }
+  else if (h->ik.c) { f = p->km->f_ik_step; control = &h->ik; }
+  void* stock[] = {&h->st, &h->es, &h->dm, &h->ds, &h->cfg, &h->opt, &actions, &reward, &done, &info, &slice_words, &slots};
+  void* with_control[] = {&h->st, &h->es, control, &h->dm, &h->ds, &h->cfg, &h->opt, &actions, &reward, &done, &info, &slice_words, &slots};
+  if (int rc = launch(h, f, p->nblocks, 32 * p->wpb, p->smem_env, stream, control ? with_control : stock)) return rc;
   if (p->reorder) {
     int N = h->N, nslots = p->nblocks * p->wpb, wpb = p->wpb;
     const int* stats = h->st.stats;
@@ -330,7 +269,7 @@ static int launch_step(fe_handle* h, const float* actions, float* reward, uint8_
   return 0;
 }
 static int plat_run_sim(fe_handle* h, int nsub, int mode, void* stream) {
-  DevScope dev(h);
+  FeDevScope dev(h);
   if (int rc = plat_prepare(h)) return rc;
   CudaPlat* p = (CudaPlat*)h->plat;
   int slice_words = h->slice_words;
@@ -340,7 +279,7 @@ static int plat_run_sim(fe_handle* h, int nsub, int mode, void* stream) {
   return 0;
 }
 static int plat_run_reset(fe_handle* h, const uint8_t* mask, void* stream) {
-  DevScope dev(h);
+  FeDevScope dev(h);
   if (int rc = plat_prepare(h)) return rc;
   CudaPlat* p = (CudaPlat*)h->plat;
   int slice_words = h->slice_words;
@@ -350,12 +289,12 @@ static int plat_run_reset(fe_handle* h, const uint8_t* mask, void* stream) {
   return 0;
 }
 static int plat_run_step(fe_handle* h, const float* actions, float* reward, uint8_t* done, int32_t* info, void* stream) {
-  DevScope dev(h);
+  FeDevScope dev(h);
   if (int rc = plat_prepare(h)) return rc;
   return launch_step(h, actions, reward, done, info, (cudaStream_t)stream);
 }
 static int plat_step_host(fe_handle* h, const float* actions, float* obs, float* reward, uint8_t* done, int32_t* info) {
-  DevScope dev(h);
+  FeDevScope dev(h);
   if (int rc = plat_prepare(h)) return rc;
   CudaPlat* p = (CudaPlat*)h->plat;
   const size_t N = h->N, ab = sizeof(float) * N * fe_action_dim(h), ob = sizeof(float) * N * h->hs.obs_dim, rb = sizeof(float) * N, ib = sizeof(int32_t) * N * FE_INFO_DIM;
@@ -380,109 +319,98 @@ static int plat_step_host(fe_handle* h, const float* actions, float* obs, float*
   if (done) memcpy(done, o + ob + rb + ib, N);
   return 0;
 }
+// device buffers of one host-side evaluation call (fe_is_aligned, fe_dense_eval, fe_ctl_eval), freed when it goes out of scope
+struct DevBufs {
+  std::vector<void*> bufs;
+  bool bad = false; // an allocation or an upload failed
+  // a device copy of `bytes` bytes at `src`, or an uninitialised output buffer when src is null
+  void* up(const void* src, size_t bytes) {
+    void* d = nullptr;
+    if (cudaMalloc(&d, bytes ? bytes : 8) != cudaSuccess) { bad = true; return nullptr; }
+    bufs.push_back(d);
+    if (src && cudaMemcpy(d, src, bytes, cudaMemcpyHostToDevice) != cudaSuccess) bad = true;
+    return d;
+  }
+  ~DevBufs() { for (void* b : bufs) cudaFree(b); }
+};
+
 static int plat_is_aligned(fe_handle* h, int n, const double* p1, const double* m1, const double* p2, const double* m2, const double* angles,
                            const int32_t* nangles, const double* thr, uint8_t* aligned, double* tq) {
-  DevScope dev(h);
+  FeDevScope dev(h);
   if (int rc = plat_prepare(h)) return rc;
   CudaPlat* p = (CudaPlat*)h->plat;
   // cos/sin of the allowed angles are evaluated on the host in float64 (the same libm the reference's numpy uses)
   std::vector<double> cs(4 * (size_t)n), sn(4 * (size_t)n);
   for (size_t i = 0; i < 4 * (size_t)n; ++i) { double a = angles[i] / 180 * 3.141592653589793; cs[i] = cos(a); sn[i] = sin(a); }
-  double *d_p1, *d_m1, *d_p2, *d_m2, *d_cs, *d_sn, *d_thr, *d_tq;
-  int32_t* d_na;
-  uint8_t* d_al;
   const size_t N = n;
-  CUDA_OK(cudaMalloc(&d_p1, 24 * N)); CUDA_OK(cudaMalloc(&d_m1, 72 * N)); CUDA_OK(cudaMalloc(&d_p2, 24 * N)); CUDA_OK(cudaMalloc(&d_m2, 72 * N));
-  CUDA_OK(cudaMalloc(&d_cs, 32 * N)); CUDA_OK(cudaMalloc(&d_sn, 32 * N)); CUDA_OK(cudaMalloc(&d_thr, 32 * N)); CUDA_OK(cudaMalloc(&d_tq, 32 * N));
-  CUDA_OK(cudaMalloc(&d_na, 4 * N)); CUDA_OK(cudaMalloc(&d_al, N));
-  cudaMemcpy(d_p1, p1, 24 * N, cudaMemcpyHostToDevice); cudaMemcpy(d_m1, m1, 72 * N, cudaMemcpyHostToDevice);
-  cudaMemcpy(d_p2, p2, 24 * N, cudaMemcpyHostToDevice); cudaMemcpy(d_m2, m2, 72 * N, cudaMemcpyHostToDevice);
-  cudaMemcpy(d_cs, cs.data(), 32 * N, cudaMemcpyHostToDevice); cudaMemcpy(d_sn, sn.data(), 32 * N, cudaMemcpyHostToDevice);
-  cudaMemcpy(d_thr, thr, 32 * N, cudaMemcpyHostToDevice); cudaMemcpy(d_na, nangles, 4 * N, cudaMemcpyHostToDevice);
+  DevBufs b;
+  void* d_p1 = b.up(p1, 24 * N);
+  void* d_m1 = b.up(m1, 72 * N);
+  void* d_p2 = b.up(p2, 24 * N);
+  void* d_m2 = b.up(m2, 72 * N);
+  void* d_cs = b.up(cs.data(), 32 * N);
+  void* d_sn = b.up(sn.data(), 32 * N);
+  void* d_na = b.up(nangles, 4 * N);
+  void* d_thr = b.up(thr, 32 * N);
+  void* d_al = b.up(nullptr, N);
+  void* d_tq = b.up(nullptr, 32 * N);
+  if (b.bad) return fail(h, -2, "fe_is_aligned: device allocation / upload failed");
   void* a[] = {&n, &d_p1, &d_m1, &d_p2, &d_m2, &d_cs, &d_sn, &d_na, &d_thr, &d_al, &d_tq};
-  int rc = launch(h, p->km->f_aligned, (n + 127) / 128, 128, 0, nullptr, a);
-  if (!rc) {
-    if (cudaMemcpy(aligned, d_al, N, cudaMemcpyDeviceToHost) != cudaSuccess || cudaMemcpy(tq, d_tq, 32 * N, cudaMemcpyDeviceToHost) != cudaSuccess)
-      rc = fail(h, -10, std::string("fe_is_aligned: ") + cudaGetErrorString(cudaGetLastError()));
-  }
-  cudaFree(d_p1); cudaFree(d_m1); cudaFree(d_p2); cudaFree(d_m2); cudaFree(d_cs); cudaFree(d_sn); cudaFree(d_thr); cudaFree(d_tq); cudaFree(d_na); cudaFree(d_al);
-  return rc;
+  if (int rc = launch(h, p->km->f_aligned, (n + 127) / 128, 128, 0, nullptr, a)) return rc;
+  if (cudaMemcpy(aligned, d_al, N, cudaMemcpyDeviceToHost) != cudaSuccess || cudaMemcpy(tq, d_tq, 32 * N, cudaMemcpyDeviceToHost) != cudaSuccess)
+    return fail(h, -10, std::string("fe_is_aligned: ") + cudaGetErrorString(cudaGetLastError()));
+  return 0;
 }
 static int plat_dense_eval(fe_handle* h, const fe_dense_config* dc, const fe_dense_recipe* rc, const double* thr, int n_goal, int n_episodes, const int32_t* first,
                            const int32_t* count, int n_records, int nsite, int npart, int act_dim, const double* spos, const double* smat, const double* ppos,
                            const uint8_t* touch, const uint8_t* reset, const uint8_t* connected, const double* ac, double* reward, uint8_t* done, double* info) {
-  DevScope dev(h);
+  FeDevScope dev(h);
   if (int rc_ = plat_prepare(h)) return rc_;
   CudaPlat* p = (CudaPlat*)h->plat;
   const size_t R = n_records, E = n_episodes;
-  std::vector<void*> bufs;
-  bool bad = false;
-  auto up = [&](const void* src, size_t bytes) -> void* {
-    void* d = nullptr;
-    if (cudaMalloc(&d, bytes ? bytes : 8) != cudaSuccess) { bad = true; return nullptr; }
-    bufs.push_back(d);
-    if (src && cudaMemcpy(d, src, bytes, cudaMemcpyHostToDevice) != cudaSuccess) bad = true;
-    return d;
-  };
-  void* d_c = up(dc, sizeof(fe_dense_config));
-  void* d_rc = up(rc, sizeof(fe_dense_recipe));
-  void* d_thr = up(thr, 32);
-  void* d_first = up(first, 4 * E);
-  void* d_count = up(count, 4 * E);
-  void* d_spos = up(spos, 24 * R * nsite);
-  void* d_smat = up(smat, 72 * R * nsite);
-  void* d_ppos = up(ppos, 24 * R * npart);
-  void* d_touch = up(touch, R * npart);
-  void* d_reset = up(reset, R);
-  void* d_conn = up(connected, R);
-  void* d_ac = up(ac, 8 * R * act_dim);
-  void* d_rew = up(nullptr, 8 * R);
-  void* d_done = up(nullptr, R);
-  void* d_info = up(nullptr, 8 * R * FE_DENSE_INFO);
-  int rcode = bad ? fail(h, -2, "fe_dense_eval: device allocation / upload failed") : 0;
-  if (!rcode) {
-    void* a[] = {&d_c, &d_rc, &d_thr, &n_goal, &n_episodes, &d_first, &d_count, &nsite, &npart, &act_dim, &d_spos, &d_smat, &d_ppos, &d_touch, &d_reset, &d_conn, &d_ac,
-                 &d_rew, &d_done, &d_info};
-    rcode = launch(h, p->km->f_dense, (n_episodes + 31) / 32, 32, 0, nullptr, a);
-  }
-  if (!rcode) {
-    if (cudaMemcpy(reward, d_rew, 8 * R, cudaMemcpyDeviceToHost) != cudaSuccess || cudaMemcpy(done, d_done, R, cudaMemcpyDeviceToHost) != cudaSuccess ||
-        cudaMemcpy(info, d_info, 8 * R * FE_DENSE_INFO, cudaMemcpyDeviceToHost) != cudaSuccess)
-      rcode = fail(h, -10, std::string("fe_dense_eval: ") + cudaGetErrorString(cudaGetLastError()));
-  }
-  for (void* b : bufs) cudaFree(b);
-  return rcode;
+  DevBufs b;
+  void* d_c = b.up(dc, sizeof(fe_dense_config));
+  void* d_rc = b.up(rc, sizeof(fe_dense_recipe));
+  void* d_thr = b.up(thr, 32);
+  void* d_first = b.up(first, 4 * E);
+  void* d_count = b.up(count, 4 * E);
+  void* d_spos = b.up(spos, 24 * R * nsite);
+  void* d_smat = b.up(smat, 72 * R * nsite);
+  void* d_ppos = b.up(ppos, 24 * R * npart);
+  void* d_touch = b.up(touch, R * npart);
+  void* d_reset = b.up(reset, R);
+  void* d_conn = b.up(connected, R);
+  void* d_ac = b.up(ac, 8 * R * act_dim);
+  void* d_rew = b.up(nullptr, 8 * R);
+  void* d_done = b.up(nullptr, R);
+  void* d_info = b.up(nullptr, 8 * R * FE_DENSE_INFO);
+  if (b.bad) return fail(h, -2, "fe_dense_eval: device allocation / upload failed");
+  void* a[] = {&d_c, &d_rc, &d_thr, &n_goal, &n_episodes, &d_first, &d_count, &nsite, &npart, &act_dim, &d_spos, &d_smat, &d_ppos, &d_touch, &d_reset, &d_conn, &d_ac,
+               &d_rew, &d_done, &d_info};
+  if (int rc_ = launch(h, p->km->f_dense, (n_episodes + 31) / 32, 32, 0, nullptr, a)) return rc_;
+  if (cudaMemcpy(reward, d_rew, 8 * R, cudaMemcpyDeviceToHost) != cudaSuccess || cudaMemcpy(done, d_done, R, cudaMemcpyDeviceToHost) != cudaSuccess ||
+      cudaMemcpy(info, d_info, 8 * R * FE_DENSE_INFO, cudaMemcpyDeviceToHost) != cudaSuccess)
+    return fail(h, -10, std::string("fe_dense_eval: ") + cudaGetErrorString(cudaGetLastError()));
+  return 0;
 }
 static int plat_ctl_eval(fe_handle* h, const fe_ctl_config* cc, int n_episodes, const int32_t* first, const int32_t* count, int n_records, const uint8_t* reset,
                          const uint8_t* policy_step, const double* action, const FeCtlIn* in, double* torques) {
-  DevScope dev(h);
+  FeDevScope dev(h);
   if (int rc_ = plat_prepare(h)) return rc_;
-  if (int rc_ = plat_module_ctl(h)) return rc_;
   CudaPlat* p = (CudaPlat*)h->plat;
   const size_t R = n_records, E = n_episodes;
-  std::vector<void*> bufs;
-  bool bad = false;
-  auto up = [&](const void* src, size_t bytes) -> void* {
-    void* d = nullptr;
-    if (cudaMalloc(&d, bytes ? bytes : 8) != cudaSuccess) { bad = true; return nullptr; }
-    bufs.push_back(d);
-    if (src && cudaMemcpy(d, src, bytes, cudaMemcpyHostToDevice) != cudaSuccess) bad = true;
-    return d;
-  };
-  void* d_c = up(cc, sizeof(fe_ctl_config));
-  void* d_first = up(first, 4 * E);
-  void* d_count = up(count, 4 * E);
-  void* d_reset = up(reset, R);
-  void* d_pol = up(policy_step, R);
-  void* d_act = up(action, 56 * R);
-  void* d_in = up(in, sizeof(FeCtlIn) * R);
-  void* d_tau = up(nullptr, 56 * R);
-  int rcode = bad ? fail(h, -2, "fe_ctl_eval: device allocation / upload failed") : 0;
-  if (!rcode) {
-    void* a[] = {&d_c, &n_episodes, &d_first, &d_count, &d_reset, &d_pol, &d_act, &d_in, &d_tau};
-    rcode = launch(h, p->km->f_ctl_eval, (n_episodes + 31) / 32, 32, 0, nullptr, a);
-  }
-  if (!rcode && cudaMemcpy(torques, d_tau, 56 * R, cudaMemcpyDeviceToHost) != cudaSuccess) rcode = fail(h, -10, std::string("fe_ctl_eval: ") + cudaGetErrorString(cudaGetLastError()));
-  for (void* b : bufs) cudaFree(b);
-  return rcode;
+  DevBufs b;
+  void* d_c = b.up(cc, sizeof(fe_ctl_config));
+  void* d_first = b.up(first, 4 * E);
+  void* d_count = b.up(count, 4 * E);
+  void* d_reset = b.up(reset, R);
+  void* d_pol = b.up(policy_step, R);
+  void* d_act = b.up(action, 56 * R);
+  void* d_in = b.up(in, sizeof(FeCtlIn) * R);
+  void* d_tau = b.up(nullptr, 56 * R);
+  if (b.bad) return fail(h, -2, "fe_ctl_eval: device allocation / upload failed");
+  void* a[] = {&d_c, &n_episodes, &d_first, &d_count, &d_reset, &d_pol, &d_act, &d_in, &d_tau};
+  if (int rc_ = launch(h, p->km->f_ctl_eval, (n_episodes + 31) / 32, 32, 0, nullptr, a)) return rc_;
+  if (cudaMemcpy(torques, d_tau, 56 * R, cudaMemcpyDeviceToHost) != cudaSuccess) return fail(h, -10, std::string("fe_ctl_eval: ") + cudaGetErrorString(cudaGetLastError()));
+  return 0;
 }

@@ -8,10 +8,8 @@
 //   fe_ik_solve        <- replaces the pybullet solve (p.calculateInverseKinematics, :177-215, :248-281; pybullet and its URDF are not
 //                         available): damped least squares on the arm's own chain, lane 0, float32 -- furniture_b200/ik.py: solve_ik is
 //                         the same algorithm in float64 (oracle/ik_oracle.py)
-// The part of an env step that follows the simulation (connect, reward, termination, observation) is the one of fe_env.h:
-// fe_ik_controls / fe_ik_finish below restate fe_env_step_one's blocks with the policy action (8 numbers) and the low-level action
-// (7 velocities + gripper) as separate arguments.  fe_env.h itself is left untouched on purpose: its step kernel is the stock build
-// that is profiled and benched (profiles/); fold the two once a capture of the folded build is taken.
+// _setup_action and everything after the simulation (connect, reward, termination, observation) are fe_env.h's fe_env_controls /
+// fe_env_finish, with the low-level action (7 velocities per arm + gripper) and the policy action as separate arguments.
 #pragma once
 #include "fe_env.h"
 
@@ -131,126 +129,6 @@ FE_HDN int fe_ik_solve(const fe_ik_config* c, const fe_ik_arm* arm, float* q, co
   return it;
 }
 
-// _setup_action + gravity compensation with the low-level action `a` (arm velocities, then the gripper action `grip`)
-FE_HD void fe_ik_controls(FeEnv* e, const float* a, float grip) {
-  FeWarp* w = e->w;
-  const fe_model* m = w->m;
-  const fe_scene* sc = e->sc;
-  const fe_config* cfg = e->cfg;
-  LANES_BEGIN
-    for (int u = lane; u < m->nu; u += 32) { // _setup_action, furniture.py:3332-3367
-      const int src = sc->act_src[u];
-      float v = src == sc->grip_action_index ? grip : a[src];
-      if (cfg->rescale_actions) v = fminf(fmaxf(v, -1.f), 1.f);
-      v *= sc->act_sign[u];
-      if (cfg->rescale_actions) {
-        const float lo = m->act_ctrlrange[u][0], hi = m->act_ctrlrange[u][1];
-        v = 0.5f * (hi + lo) + 0.5f * (hi - lo) * v;
-      }
-      w->ctrl()[u] = v;
-    }
-    for (int i = lane; i < sc->narm; i += 32) w->qfrc_applied()[sc->arm_dof[i]] = w->bias()[sc->arm_dof[i]]; // gravity compensation, :3372-3377
-    for (int i = lane; i < sc->ngrip; i += 32) w->qfrc_applied()[sc->grip_dof[i]] = w->bias()[sc->grip_dof[i]];
-    if (lane == 0) { e->ei[0] = 0; e->ei[1] = -1; e->ei[6] = 0; w->u()[2] = 0; }
-  LANES_END
-}
-
-// what follows the simulation in FurnitureEnv.step, with the policy action `a` (act_dim numbers) for reward and connect
-// `fail`: some _do_simulation of this step raised; `reset_now`: the last one did, so the env has not been reset for it yet
-FE_HD void fe_ik_finish(FeEnv* e, const float* a, int act_dim, float connect, int fail, int reset_now, float* reward_out, uint8_t* done_out, int32_t* info_out) {
-  FeWarp* w = e->w;
-  const fe_model* m = w->m;
-  const fe_scene* sc = e->sc;
-  const fe_config* cfg = e->cfg;
-  const int np = m->npart, env = e->env;
-  FE_SYNC;
-  if (reset_now) {
-    fe_env_reset_one(e);
-  } else {
-    if (connect > 0.f) { // furniture.py:1290-1322: per arm, the first part both of its fingers touch; stop at the first connection
-      for (int arm = 0; arm < sc->narms; ++arm) {
-        const int both = arm == 0 ? 3 : 24;
-        int part = -1;
-        for (int p = 0; p < np; ++p) if ((w->touch()[p] & both) == both) { part = p; break; }
-        if (part >= 0) {
-          fe_try_connect_scan(e, part);
-          if (e->ei[0]) { fe_connect(e); break; }
-        }
-      }
-    }
-    const int repin = e->ei[1];
-    FE_SYNC; // every lane has read the flag before lane 0 clears it
-    if (repin >= 0) { // furniture.py:426-436: re-pin the merged group at the recorded pose, one more step
-      LANES_BEGIN
-        if (lane == 0) {
-          const int b1 = e->ei[1], qa = m->link_qadr[m->nrlink + b1];
-          double tr[3] = {e->ed[4] - (double)w->qpos()[qa], e->ed[5] - (double)w->qpos()[qa + 1], e->ed[6] - (double)w->qpos()[qa + 2]};
-          fe_move_group(e, b1, tr, e->ed + 7, 0.f);
-          e->ei[1] = -1;
-        }
-      LANES_END
-      fe_fwd_step(e);
-      if (w->u()[2] & 8) { fail = 1; fe_env_reset_one(e); }
-    }
-  }
-  // reward (furniture.py:482-541), termination (:440-445, :451-480)
-  LANES_BEGIN
-    if (lane == 0) {
-      float touch_r = 0.f, pick_r = 0.f;
-      int* touched = e->es.touched + (size_t)env * np;
-      int* picked = e->es.picked + (size_t)env * np;
-      if (!fail)
-        for (int arm = 0; arm < sc->narms; ++arm) // furniture.py:492-523: both fingers of the same arm
-          for (int p = 0; p < np; ++p) {
-            const int t = w->touch()[p], both = arm == 0 ? 3 : 24;
-            if ((t & both) == both) {
-              if (!touched[p]) { touched[p] = 1; touch_r += cfg->touch_reward; }
-              if (!(t & 4) && !picked[p]) { picked[p] = 1; pick_r += cfg->pick_reward; }
-            }
-          }
-      const int nc = e->es.num_connected[env];
-      const float success_r = cfg->success_reward * (float)(nc - e->es.prev_num_connected[env]);
-      const int connected_now = nc != e->es.prev_num_connected[env]; // _connected: a connection was made during this step
-      e->es.prev_num_connected[env] = nc;
-      float sq = 0.f;
-      for (int k = 0; k < act_dim; ++k) sq += a[k] * a[k];
-      float reward = success_r + touch_r + pick_r - cfg->ctrl_penalty_coef * sq;
-      int success = (nc == np - 1 && np > 1) ? 1 : 0;
-      int done = success;
-      if (e->es.dense) { // FurnitureSawyerEnv._step: reward, _done, info = _compute_reward(a); done = done or _done (furniture_sawyer.py:66-84)
-        FeSliceWorld world = {w};
-        const double thr[4] = {cfg->alignment_pos_dist, cfg->alignment_rot_dist_up, cfg->alignment_rot_dist_forward, cfg->alignment_project_dist};
-        double ad[FE_MAXU + 2], dr = 0.0, di[FE_DENSE_INFO];
-        for (int k = 0; k < act_dim; ++k) ad[k] = (double)a[k];
-        int dd = 0;
-        FeDenseState* ds = e->es.dstate + env;
-        fe_dense_step(world, e->es.dense, &sc->dense, thr, np - 1, ds, ad, act_dim, connected_now, &dr, &dd, di);
-        reward = (float)dr;
-        success = ds->success;
-        done = done || dd;
-        float* dinf = e->es.dinfo + (size_t)env * FE_DENSE_INFO;
-        for (int k = 0; k < FE_DENSE_INFO; ++k) dinf[k] = (float)di[k];
-      }
-      const int len = ++e->es.episode_len[env];
-      float penalty = 0.f;
-      if (len == cfg->max_episode_steps || fail) { done = 1; if (fail) penalty = -cfg->unstable_penalty_coef; }
-      reward += penalty;
-      reward_out[env] = reward;
-      done_out[env] = (uint8_t)done;
-      if (e->es.packed) { float* pk = e->es.packed + (size_t)env * (sc->obs_dim + 2) + sc->obs_dim; pk[0] = reward; pk[1] = done ? 1.f : 0.f; }
-      int32_t* info = info_out + (size_t)env * FE_INFO_DIM;
-      info[0] = nc; info[1] = success; info[2] = fail; info[3] = len; info[4] = w->u()[0]; info[5] = w->u()[3];
-      e->es.done[env] = done;
-      // An unstable episode resets twice, as the reference does: once inside _do_simulation's except branch
-      // (furniture.py:2889-2897) and once more by the VecEnv worker because the step returned done (subproc_vec_env.py:16-20).
-      // The second reset zeroes the episode length that _after_step just incremented and consumes its own random draws,
-      // so the env's generator stays draw-for-draw on the reference's stream.
-      e->ei[6] = done;
-    }
-  LANES_END
-  if (e->ei[6]) fe_env_reset_one(e); else fe_write_obs(e);
-}
-
 // first get_control of the step (lane 0), one arm: hand pose of the last forward pass -> targets -> joint command -> first velocities.
 // `a` points at this arm's (move, rotate) numbers
 FE_HDN void fe_ik_command(FeEnv* e, const FeIkArgs& ik, int arm_i, const float* a) {
@@ -346,7 +224,7 @@ FE_FN void fe_env_ik_step_one(FeEnv* e, FeIkArgs ik, const float* action, float*
         if (lane < 7 * na) st->low[lane] = fminf(fmaxf(-c->kp * (w->qpos()[c->arm[lane / 7].arm_qadr[lane % 7]] - st->q_cmd[lane]), -1.f), 1.f);
       LANES_END
     }
-    fe_ik_controls(e, st->low, grip);
+    fe_env_controls(e, st->low, grip);
     for (int i = 0; i < e->cfg->nsub; ++i) fe_substep_lockstep(w);
     if (w->u()[2] & 8) { // _do_simulation's except branch: reset, then the remaining repeats run on the new episode (furniture.py:2889-2897)
       fail = 1;
@@ -354,5 +232,5 @@ FE_FN void fe_env_ik_step_one(FeEnv* e, FeIkArgs ik, const float* action, float*
       if (r + 1 < c->action_repeat) fe_env_reset_one(e); else reset_now = 1;
     }
   }
-  fe_ik_finish(e, a, act_dim, connect, fail, reset_now, reward_out, done_out, info_out);
+  fe_env_finish(e, a, act_dim, connect, fail, reset_now, reward_out, done_out, info_out);
 }

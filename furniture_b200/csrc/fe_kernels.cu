@@ -7,7 +7,8 @@
 #include <stdint.h>
 
 #include "../../include/furniture_b200.h"
-#include "fe_env.h"
+#include "fe_ik.h"
+#include "fe_ctl.h"
 
 // ---------------------------------------------------------------- kernels
 
@@ -18,19 +19,32 @@ extern "C" __global__ void __launch_bounds__(32 * FE_MAX_WPB) fe_sim_kernel(FeSt
   fe_run_env(s, m, opt, env, nsub, mode, fe_smem + (size_t)wib * slice_words, dbg);
 }
 
+// the step kernels, one per control type: same launch shape, envs packed into blocks by fe_order_kernel
 extern "C" __global__ void __launch_bounds__(32 * FE_MAX_WPB) fe_env_step_kernel(FeState st, FeEnvState es, const fe_model* __restrict__ m, const fe_scene* __restrict__ sc,
                                                          fe_config cfg, FeOpt opt, const float* __restrict__ actions, float* reward, uint8_t* done,
                                                          int32_t* info, int slice_words, const int* __restrict__ slots) {
   const int wib = threadIdx.x >> 5, slot = blockIdx.x * (blockDim.x >> 5) + wib;
   const int env = slots[slot];
   if (env < 0) return; // unused slot (blocks of heavy envs are deliberately left partly empty)
-  FeEnv e;
-  fe_env_bind(&e, fe_smem + (size_t)wib * (slice_words + FE_ENV_EXTRA_WORDS), m, sc, &cfg, opt, st, es, env, slice_words);
-  fe_load(e.w, st, env);
-  fe_env_load_groups(&e);
-  fe_env_step_one(&e, actions, reward, done, info);
-  fe_env_store_groups(&e);
-  fe_store(e.w, st, env);
+  fe_env_run(fe_smem + (size_t)wib * (slice_words + FE_ENV_EXTRA_WORDS), m, sc, &cfg, opt, st, es, env, slice_words, [&](FeEnv* e) { fe_env_step_one(e, actions, reward, done, info); });
+}
+
+extern "C" __global__ void __launch_bounds__(32 * FE_MAX_WPB) fe_env_ik_step_kernel(FeState st, FeEnvState es, FeIkArgs ik, const fe_model* __restrict__ m,
+                                                            const fe_scene* __restrict__ sc, fe_config cfg, FeOpt opt, const float* __restrict__ actions,
+                                                            float* reward, uint8_t* done, int32_t* info, int slice_words, const int* __restrict__ slots) {
+  const int wib = threadIdx.x >> 5, slot = blockIdx.x * (blockDim.x >> 5) + wib;
+  const int env = slots[slot];
+  if (env < 0) return; // unused slot (blocks of heavy envs are deliberately left partly empty)
+  fe_env_run(fe_smem + (size_t)wib * (slice_words + FE_ENV_EXTRA_WORDS), m, sc, &cfg, opt, st, es, env, slice_words, [&](FeEnv* e) { fe_env_ik_step_one(e, ik, actions, reward, done, info); });
+}
+
+extern "C" __global__ void __launch_bounds__(32 * FE_MAX_WPB) fe_env_ctl_step_kernel(FeState st, FeEnvState es, FeCtlArgs ctl, const fe_model* __restrict__ m,
+                                                             const fe_scene* __restrict__ sc, fe_config cfg, FeOpt opt, const float* __restrict__ actions,
+                                                             float* reward, uint8_t* done, int32_t* info, int slice_words, const int* __restrict__ slots) {
+  const int wib = threadIdx.x >> 5, slot = blockIdx.x * (blockDim.x >> 5) + wib;
+  const int env = slots[slot];
+  if (env < 0) return; // unused slot (blocks of heavy envs are deliberately left partly empty)
+  fe_env_run(fe_smem + (size_t)wib * (slice_words + FE_ENV_EXTRA_WORDS), m, sc, &cfg, opt, st, es, env, slice_words, [&](FeEnv* e) { fe_env_ctl_step_one(e, ctl, actions, reward, done, info); });
 }
 
 extern "C" __global__ void __launch_bounds__(32 * FE_MAX_WPB) fe_env_reset_kernel(FeState st, FeEnvState es, const fe_model* __restrict__ m, const fe_scene* __restrict__ sc,
@@ -38,13 +52,7 @@ extern "C" __global__ void __launch_bounds__(32 * FE_MAX_WPB) fe_env_reset_kerne
   const int wib = threadIdx.x >> 5, env = blockIdx.x * (blockDim.x >> 5) + wib;
   if (env >= st.N) return;
   if (mask && !mask[env]) return;
-  FeEnv e;
-  fe_env_bind(&e, fe_smem + (size_t)wib * (slice_words + FE_ENV_EXTRA_WORDS), m, sc, &cfg, opt, st, es, env, slice_words);
-  fe_load(e.w, st, env);
-  fe_env_load_groups(&e);
-  fe_env_reset_one(&e);
-  fe_env_store_groups(&e);
-  fe_store(e.w, st, env);
+  fe_env_run(fe_smem + (size_t)wib * (slice_words + FE_ENV_EXTRA_WORDS), m, sc, &cfg, opt, st, es, env, slice_words, [&](FeEnv* e) { fe_env_reset_one(e); });
 }
 
 // Packs the envs into blocks for the next step from the work their last step took (cycles in the five phases, barrier
@@ -112,4 +120,12 @@ extern "C" __global__ void fe_dense_eval_kernel(const fe_dense_config* c, const 
   const int e = blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= n_episodes) return;
   fe_dense_eval_episode(c, rc, thr, n_goal, first[e], count[e], nsite, npart, act_dim, spos, smat, ppos, touch, reset, connected, ac, reward, done, info);
+}
+
+// test hook of the torque controllers' arithmetic (fe_ctl_eval): one thread per episode of records
+extern "C" __global__ void fe_ctl_eval_kernel(const fe_ctl_config* c, int n_episodes, const int32_t* first, const int32_t* count, const uint8_t* reset,
+                                   const uint8_t* policy_step, const double* action, const FeCtlIn* in, double* tau) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= n_episodes) return;
+  fe_ctl_eval_episode(c, first[e], count[e], reset, policy_step, action, in, tau);
 }

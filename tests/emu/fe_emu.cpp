@@ -46,32 +46,19 @@ static int plat_run_sim(fe_handle* h, int nsub, int mode, void*) {
 static int plat_run_reset(fe_handle* h, const uint8_t* mask, void*) {
   fe_h_lay = h->lay;
   std::vector<double> slice((h->slice_words + FE_ENV_EXTRA_WORDS) / 2 + 8);
-  for (int env = 0; env < h->N; ++env) {
-    if (mask && !mask[env]) continue;
-    FeEnv e;
-    fe_env_bind(&e, (float*)slice.data(), h->dm, h->ds, &h->cfg, h->opt, h->st, h->es, env, h->slice_words);
-    fe_load(e.w, h->st, env);
-    fe_env_load_groups(&e);
-    fe_env_reset_one(&e);
-    fe_env_store_groups(&e);
-    fe_store(e.w, h->st, env);
-  }
+  for (int env = 0; env < h->N; ++env)
+    if (!mask || mask[env]) fe_env_run((float*)slice.data(), h->dm, h->ds, &h->cfg, h->opt, h->st, h->es, env, h->slice_words, [&](FeEnv* e) { fe_env_reset_one(e); });
   return 0;
 }
 static int plat_run_step(fe_handle* h, const float* actions, float* reward, uint8_t* done, int32_t* info, void*) {
   fe_h_lay = h->lay;
   std::vector<double> slice((h->slice_words + FE_ENV_EXTRA_WORDS) / 2 + 8);
-  for (int env = 0; env < h->N; ++env) {
-    FeEnv e;
-    fe_env_bind(&e, (float*)slice.data(), h->dm, h->ds, &h->cfg, h->opt, h->st, h->es, env, h->slice_words);
-    fe_load(e.w, h->st, env);
-    fe_env_load_groups(&e);
-    if (h->ctl.c) fe_env_ctl_step_one(&e, h->ctl, actions, reward, done, info);
-    else if (h->ik.c) fe_env_ik_step_one(&e, h->ik, actions, reward, done, info);
-    else fe_env_step_one(&e, actions, reward, done, info);
-    fe_env_store_groups(&e);
-    fe_store(e.w, h->st, env);
-  }
+  for (int env = 0; env < h->N; ++env)
+    fe_env_run((float*)slice.data(), h->dm, h->ds, &h->cfg, h->opt, h->st, h->es, env, h->slice_words, [&](FeEnv* e) {
+      if (h->ctl.c) fe_env_ctl_step_one(e, h->ctl, actions, reward, done, info);
+      else if (h->ik.c) fe_env_ik_step_one(e, h->ik, actions, reward, done, info);
+      else fe_env_step_one(e, actions, reward, done, info);
+    });
   return 0;
 }
 static int plat_step_host(fe_handle* h, const float* actions, float* obs, float* reward, uint8_t* done, int32_t* info) {
