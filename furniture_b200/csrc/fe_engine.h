@@ -15,10 +15,6 @@
 #include "fe_collide.h"
 #include "fe_model.h"
 #include "fe_warp.h"
-#if !FE_DEVICE_BUILD
-#include <stdio.h>
-#include <stdlib.h>
-#endif
 
 #define FE_MINVAL 1e-15f
 #define FE_MINIMP 0.0001f
@@ -36,7 +32,6 @@ struct FeOpt {
   int newton_iters; // max Newton iterations
   int ls_iters;     // max line-search evaluations
   float tolerance;  // scaled improvement / gradient tolerance (MuJoCo: 1e-8 in double)
-  int lockstep;     // bit k: block barrier before phase k of fe_substep_lockstep (instruction-fetch sharing)
 };
 
 // ---- shared-memory slice of one warp (= one env).  All sizes in 4-byte words.
@@ -76,7 +71,7 @@ __constant__ FeLayout fe_c_lay;
 #define FE_LAY fe_h_lay
 #endif
 
-#define FE_WARP_HDR_WORDS 10
+#define FE_WARP_HDR_WORDS 10 /* sizeof(FeWarp) is 8 words; the 2 spare words keep every array at the offset the kernels were tuned with */
 struct FeWarp { // header at word 0 of the slice
   const fe_model* m;
   FeOpt opt;
@@ -245,54 +240,6 @@ FE_FN void fe_chol_solve(FeWarp* w, const float* L, const int* first, int n, flo
       for (int j = fk + lane; j < k; j += 32) tmp[j] -= L[fe_tri(k) + j] * xk;
     LANES_END
   }
-}
-
-// The same factorisation and solves done by lane 0 alone in tight loops (envelope-aware, 4 partial sums to pipeline the
-// slice loads).  For the small systems of this solver the barriers and per-column regions of the cooperative version cost
-// more than the arithmetic they spread, and a short loop stays in the instruction cache.
-FE_FN bool fe_chol_serial(FeWarp* w, float* H, const int* first, int n, const int* skip, float* x, float* tmp) {
-  int ok = 1;
-  LANES_BEGIN
-    if (lane == 0) {
-      for (int i = 0; i < n; ++i) {
-        if (skip && skip[i]) continue;
-        float* Hi = H + fe_tri(i);
-        const int fi = first[i];
-        for (int k = fi; k <= i; ++k) {
-          if (skip && skip[k]) { continue; }
-          const float* Hk = H + fe_tri(k);
-          const int fk = first[k], j0 = fi > fk ? fi : fk;
-          float s0 = Hi[k], s1 = 0.f, s2 = 0.f, s3 = 0.f;
-          int j = j0;
-          for (; j + 3 < k; j += 4) { s0 -= Hi[j] * Hk[j]; s1 -= Hi[j + 1] * Hk[j + 1]; s2 -= Hi[j + 2] * Hk[j + 2]; s3 -= Hi[j + 3] * Hk[j + 3]; }
-          for (; j < k; ++j) s0 -= Hi[j] * Hk[j];
-          float s = (s0 + s1) + (s2 + s3);
-          if (k < i) Hi[k] = s / Hk[k];
-          else { if (!(s > 1e-30f)) { ok = 0; s = 1e-30f; } Hi[i] = sqrtf(s); }
-        }
-      }
-      // forward: tmp = L^-1 x
-      for (int i = 0; i < n; ++i) {
-        if (skip && skip[i]) continue;
-        const float* Hi = H + fe_tri(i);
-        float s0 = x[i], s1 = 0.f;
-        int j = first[i];
-        for (; j + 1 < i; j += 2) { s0 -= Hi[j] * tmp[j]; s1 -= Hi[j + 1] * tmp[j + 1]; }
-        for (; j < i; ++j) s0 -= Hi[j] * tmp[j];
-        tmp[i] = (s0 + s1) / Hi[i];
-      }
-      // backward: x = L^-T tmp (column sweep)
-      for (int i = n - 1; i >= 0; --i) {
-        if (skip && skip[i]) continue;
-        const float* Hi = H + fe_tri(i);
-        const float xi = tmp[i] / Hi[i];
-        x[i] = xi;
-        for (int j = first[i]; j < i; ++j) tmp[j] -= Hi[j] * xi;
-      }
-      w->iscr()[0] = ok;
-    }
-  LANES_END
-  return w->iscr()[0] != 0;
 }
 
 // Free-part blocks whose rows start at their own block and that no later row reaches are independent 6x6 systems:
@@ -1673,12 +1620,7 @@ FE_FN void fe_newton_regs(FeWarp* w, int nA) {
 
 // cooperative Newton solve over the active scope (w->nact dofs; in FAST scope the free parts are excluded)
 FE_FN void fe_solve_coop(FeWarp* w) {
-#if FE_DEVICE_BUILD
-#define FE_CTICK(slot) { long long t1_ = clock64(); if ((threadIdx.x & 31u) == 0) w->u()[slot] += (int)((t1_ - t0_) >> 4); t0_ = t1_; }
-  long long t0_ = clock64();
-#else
-#define FE_CTICK(slot)
-#endif
+  FE_TICK_START
   const fe_model* m = w->m;
   const int nr = m->nr, nrl = m->nrlink, np = w->fast ? 0 : m->npart, nv = w->nact, ncon = w->u()[0], ne = w->fast ? 0 : m->neq;
   const bool fast = w->fast != 0;
@@ -1754,19 +1696,15 @@ FE_FN void fe_solve_coop(FeWarp* w) {
     }
   LANES_END
   const int nA = w->iscr()[31];
-#if !FE_DEVICE_BUILD
-  if (getenv("FE_DEBUG_SOLVE")) { printf("  coupled flags:"); for (int p = 0; p < np; ++p) printf(" %d(cnt %d)", w->iscr()[p], w->plist()[9 * p + 8]); printf(" kinds:"); for (int c = 0; c < ncon; ++c) printf(" %d", w->c_kind()[c]); printf("\n"); }
-#endif
-  bool regs = nA <= 32 && !(w->opt.lockstep & 512);
-  const bool serial = (w->opt.lockstep & 256) != 0;
+  bool regs = nA <= 32;
   if (!fast) for (int p = 0; p < m->npart; ++p) if (w->plist()[9 * p + 8] > 8) regs = false; // needs the grouped static-contact path
   int iter = 0;
   float cost = 0.f, impr = 0.f;
-  FE_CTICK(25)
+  FE_TICK(w->u(), 25)
   for (;;) {
     const float ccost = fe_update(w);
     fe_mul_JT(w, w->fc());
-    FE_CTICK(26)
+    FE_TICK(w->u(), 26)
     LANES_BEGIN
       float s = 0.f, gsq = 0.f;
       for (int i = lane; i < nv; i += 32) {
@@ -1780,22 +1718,19 @@ FE_FN void fe_solve_coop(FeWarp* w) {
     LANES_END
     const float gauss = fe_sum32(w->scr()), gnorm = sqrtf(fe_sum32(w->scr() + 32));
     cost = gauss + ccost;
-#if !FE_DEVICE_BUILD
-    if (getenv("FE_DEBUG_SOLVE")) printf("  coop it %d nact %d active %d regs %d cost %.9g gnorm %.4g scaled-g %.3g impr %.3g\n", iter, nv, nA, (int)regs, cost, gnorm, scale * gnorm, scale * impr);
-#endif
     if (!(cost == cost)) { LANES_BEGIN if (lane == 0) w->u()[2] |= 2; LANES_END break; }
     // MuJoCo stops on scale*(oldcost - cost) < tol; in fp32 that difference of two large costs is round-off, so the
     // improvement is taken from the line search instead: -alpha p'(0) / 2 (exact for a quadratic, the Newton decrement)
     if (iter > 0) { if (scale * impr < w->opt.tolerance || scale * gnorm < w->opt.tolerance) break; }
     else if (scale * gnorm < w->opt.tolerance) break;
     if (iter >= w->opt.newton_iters) break;
-    FE_CTICK(27)
+    FE_TICK(w->u(), 27)
     fe_build_H(w, regs);
-    FE_CTICK(28)
+    FE_TICK(w->u(), 28)
     if (regs) {
       LANES_BEGIN for (int i = lane; i < nv; i += 32) w->search()[i] = -w->grad()[i]; LANES_END
       if (!fast) { fe_chol_blocks(w, w->H(), w->skip()); fe_solve_blocks(w, w->H(), w->skip(), w->search()); }
-      FE_CTICK(29)
+      FE_TICK(w->u(), 29)
       if (nA <= 16) fe_newton_regs<16>(w, nA); else if (nA <= 24) fe_newton_regs<24>(w, nA); else fe_newton_regs<32>(w, nA);
     } else {
       const int* skip = nullptr;
@@ -1806,16 +1741,11 @@ FE_FN void fe_solve_coop(FeWarp* w) {
       }
       LANES_BEGIN for (int i = lane; i < nv; i += 32) w->search()[i] = -w->grad()[i]; LANES_END
       if (skip) fe_solve_blocks(w, w->H(), skip, w->search());
-      if (serial) {
-        if (!fe_chol_serial(w, w->H(), w->first(), nv, skip, w->search(), w->Mv())) { LANES_BEGIN if (lane == 0) w->u()[2] |= 4; LANES_END }
-        FE_CTICK(29)
-      } else {
-        if (!fe_chol(w, w->H(), w->first(), nv, skip)) { LANES_BEGIN if (lane == 0) w->u()[2] |= 4; LANES_END }
-        FE_CTICK(29)
-        fe_chol_solve(w, w->H(), w->first(), nv, w->search(), w->Mv(), skip);
-      }
+      if (!fe_chol(w, w->H(), w->first(), nv, skip)) { LANES_BEGIN if (lane == 0) w->u()[2] |= 4; LANES_END }
+      FE_TICK(w->u(), 29)
+      fe_chol_solve(w, w->H(), w->first(), nv, w->search(), w->Mv(), skip);
     }
-    FE_CTICK(30)
+    FE_TICK(w->u(), 30)
     fe_mul_M(w, w->search(), w->Mv());
     fe_mul_J(w, w->search(), w->c_jv(), w->w_jv(), w->l_jv(), false);
     LANES_BEGIN
@@ -1845,7 +1775,7 @@ FE_FN void fe_solve_coop(FeWarp* w) {
       dxold = fabsf(next - alpha);
       alpha = next;
     }
-    FE_CTICK(31)
+    FE_TICK(w->u(), 31)
     if (!(alpha > 0.f)) break;
     impr = -0.5f * alpha * p1_0;
     LANES_BEGIN
@@ -1865,8 +1795,7 @@ FE_FN void fe_solve_coop(FeWarp* w) {
   fe_update(w);
   fe_mul_JT(w, w->fc());
   LANES_BEGIN if (lane == 0) { if (iter > w->u()[3]) w->u()[3] = iter; w->u()[7] += iter; } LANES_END
-  FE_CTICK(25)
-#undef FE_CTICK
+  FE_TICK(w->u(), 25)
 }
 
 
@@ -2223,12 +2152,7 @@ FE_FN void fe_solve_robot_limits(FeWarp* w) {
 FE_FN void fe_solve(FeWarp* w) {
   const fe_model* m = w->m;
   const int ncon = w->u()[0], ne = m->neq, np = m->npart, nrl = m->nrlink, nr = m->nr;
-#if FE_DEVICE_BUILD
-#define FE_STICK(slot) { long long t1_ = clock64(); if ((threadIdx.x & 31u) == 0) w->u()[slot] += (int)((t1_ - t0_) >> 4); t0_ = t1_; }
-  long long t0_ = clock64();
-#else
-#define FE_STICK(slot)
-#endif
+  FE_TICK_START
   LANES_BEGIN
     int rcon = 0, cpl = 0;
     for (int c = lane; c < ncon; c += 32) { const int k = w->c_kind()[c]; rcon |= (k == 1 || k == 2); }
@@ -2250,10 +2174,7 @@ FE_FN void fe_solve(FeWarp* w) {
     if (lane == 0) w->u()[3] = 0;
   LANES_END
   const unsigned cplmask = fe_ballot32(w->iscr());
-  bool robot_in = fe_ballot32(w->colmap()) != 0u;
-#if !FE_DEVICE_BUILD
-  if (getenv("FE_NO_RLIM")) robot_in = true;
-#endif
+  const bool robot_in = fe_ballot32(w->colmap()) != 0u;
   if (cplmask == 0u && !robot_in) { // nothing couples two moving blocks and the robot touches nothing
     fe_solve_parts_grouped(w, 0u);
     LANES_BEGIN
@@ -2293,18 +2214,18 @@ FE_FN void fe_solve(FeWarp* w) {
     ncc += w->iscr()[30];
     LANES_BEGIN LANES_END
   }
-  if (nA <= 32 && ncc <= 32 && !(w->opt.lockstep & 1024)) {
-    FE_STICK(21)
+  if (nA <= 32 && ncc <= 32) {
+    FE_TICK(w->u(), 21)
     fe_solve_parts_grouped(w, cplmask);
     LANES_BEGIN
       if (lane == 0) { int mx = 0; for (int p = 0; p < np; ++p) if (!((cplmask >> p) & 1u)) mx = w->iscr()[p] > mx ? w->iscr()[p] : mx; w->u()[3] = mx; w->u()[4] += mx; }
     LANES_END
     if (!robot_in) fe_solve_robot_limits(w);
-    FE_STICK(22)
+    FE_TICK(w->u(), 22)
     if (nA <= 16) fe_solve_comp<16>(w, nA, ncc, cplmask, robot_in ? 1 : 0);
     else if (nA <= 24) fe_solve_comp<24>(w, nA, ncc, cplmask, robot_in ? 1 : 0);
     else fe_solve_comp<32>(w, nA, ncc, cplmask, robot_in ? 1 : 0);
-    FE_STICK(23)
+    FE_TICK(w->u(), 23)
     return;
   }
   // fallback: cooperative solver in shared memory (all dofs when something couples, else the robot block)
@@ -2318,7 +2239,6 @@ FE_FN void fe_solve(FeWarp* w) {
   }
   fe_solve_coop(w);
   LANES_BEGIN if (lane == 0) { w->fast = 0; w->nact = m->nv; } LANES_END
-#undef FE_STICK
 }
 
 // ---------------------------------------------------------------- mj_Euler + mj_advance
@@ -2392,24 +2312,15 @@ FE_FN void fe_substep(FeWarp* w) {
 // same time, which is what keeps the instruction cache effective for this large, mostly straight-line code.  Only legal
 // where every live warp of the block executes the same number of steps (the nsub loop of an env step).
 FE_FN void fe_substep_lockstep(FeWarp* w) {
-  const int ls = w->opt.lockstep;
-#if FE_DEVICE_BUILD
-#define FE_TICK(slot) { long long t1_ = clock64(); if ((threadIdx.x & 31u) == 0) w->u()[slot] += (int)((t1_ - t0_) >> 4); t0_ = t1_; }
-#define FE_TICKB(slot) { long long t1_ = clock64(); if ((threadIdx.x & 31u) == 0) { w->u()[13] += (int)((t1_ - t0_) >> 4); w->u()[slot] += (int)((t1_ - t0_) >> 4); } t0_ = t1_; }
-  long long t0_ = clock64();
-#else
-#define FE_TICK(slot)
-#define FE_TICKB(slot)
-#endif
-  if (ls & 1) { FE_BLOCK_SYNC; } FE_TICKB(16) fe_kin_smooth(w); FE_TICK(8)
-  if (ls & 2) { FE_BLOCK_SYNC; } FE_TICKB(17) fe_collide(w); FE_TICK(9)
-  if (ls & 4) { FE_BLOCK_SYNC; } FE_TICKB(18) fe_assemble(w); FE_TICK(10)
-  if (ls & 8) { FE_BLOCK_SYNC; } FE_TICKB(19) fe_solve(w);
+  // the wait at each barrier is counted in slot 13 (all barriers) and in the barrier's own slot 16-20
+  FE_TICK_START
+  FE_BLOCK_SYNC; FE_TICK(w->u(), 13, 16) fe_kin_smooth(w); FE_TICK(w->u(), 8)
+  FE_BLOCK_SYNC; FE_TICK(w->u(), 13, 17) fe_collide(w); FE_TICK(w->u(), 9)
+  FE_BLOCK_SYNC; FE_TICK(w->u(), 13, 18) fe_assemble(w); FE_TICK(w->u(), 10)
+  FE_BLOCK_SYNC; FE_TICK(w->u(), 13, 19) fe_solve(w);
 #if FE_DEVICE_BUILD
   { const int d_ = (int)((clock64() - t0_) >> 4); if ((threadIdx.x & 31u) == 0 && d_ > w->u()[15]) w->u()[15] = d_; }
 #endif
-  FE_TICK(11)
-  if (ls & 16) { FE_BLOCK_SYNC; } FE_TICKB(20) fe_integrate(w); FE_TICK(12)
-#undef FE_TICK
-#undef FE_TICKB
+  FE_TICK(w->u(), 11)
+  FE_BLOCK_SYNC; FE_TICK(w->u(), 13, 20) fe_integrate(w); FE_TICK(w->u(), 12)
 }

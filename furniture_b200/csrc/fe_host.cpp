@@ -101,10 +101,8 @@ struct CudaPlat {
   FeModule* km = nullptr;
   size_t smem_sim = 0, smem_env = 0;
   int wpb = 1;
-  int reorder = 1, heavy_k = 7, heavy_shift = 18; // heavy: 2^(18/16) = 2.2x the median work; 7 of the 14 warp slots used
   int* slots = nullptr;  // block slot -> env (or -1)
   float* pred = nullptr; // per env: predicted work of the next step
-  float decay = 0.85f;
   int nblocks = 0;
   float* pin_act = nullptr;
   unsigned char* pin_out = nullptr;
@@ -182,22 +180,16 @@ static int plat_prepare(fe_handle* h) {
   CudaPlat* p = (CudaPlat*)h->plat;
   if (int rc = plat_module(h)) return rc;
   if (p->smem_sim) return 0;
-  // warps (= envs) per block: as many as fit in 227 KB of shared memory, at most FE_MAX_WPB; FE_WPB overrides
+  // warps (= envs) per block: as many as fit in 227 KB of shared memory, at most FE_MAX_WPB
   const size_t per_env = (size_t)(h->slice_words + FE_ENV_EXTRA_WORDS) * 4;
   int wpb = (int)((227 * 1024 - 1024) / per_env);
   if (wpb > FE_MAX_WPB) wpb = FE_MAX_WPB;
-  if (const char* e = getenv("FE_WPB")) { int v = atoi(e); if (v >= 1 && v <= wpb) wpb = v; }
   if (wpb < 1) return fail(h, -11, "model does not fit in shared memory");
   p->wpb = wpb;
-  if (const char* e = getenv("FE_REORDER")) p->reorder = atoi(e);
-  if (const char* e = getenv("FE_HEAVY_K")) p->heavy_k = atoi(e);
-  if (const char* e = getenv("FE_HEAVY_SHIFT")) p->heavy_shift = atoi(e);
-  if (p->heavy_k >= wpb) p->heavy_k = wpb / 2;
   p->nblocks = (h->N + wpb - 1) / wpb + FE_EXTRA_BLOCKS;
   {
     std::vector<int> init((size_t)p->nblocks * wpb, -1);
     for (int i = 0; i < h->N; ++i) init[i] = i;
-    if (const char* e = getenv("FE_PRED_DECAY")) p->decay = 0.01f * (float)atoi(e);
     CUDA_OK(cudaMalloc((void**)&p->pred, sizeof(float) * (size_t)h->N));
     CUDA_OK(cudaMemset(p->pred, 0, sizeof(float) * (size_t)h->N));
     CUDA_OK(cudaMalloc((void**)&p->slots, sizeof(int) * init.size()));
@@ -257,14 +249,11 @@ static int launch_step(fe_handle* h, const float* actions, float* reward, uint8_
   void* stock[] = {&h->st, &h->es, &h->dm, &h->ds, &h->cfg, &h->opt, &actions, &reward, &done, &info, &slice_words, &slots};
   void* with_control[] = {&h->st, &h->es, control, &h->dm, &h->ds, &h->cfg, &h->opt, &actions, &reward, &done, &info, &slice_words, &slots};
   if (int rc = launch(h, f, p->nblocks, 32 * p->wpb, p->smem_env, stream, control ? with_control : stock)) return rc;
-  if (p->reorder) {
-    int N = h->N, nslots = p->nblocks * p->wpb, wpb = p->wpb;
-    const int* stats = h->st.stats;
-    int* order = h->st.order;
-    int* sl = p->slots;
-    void* b[] = {&N, &stats, &order, &sl, &nslots, &wpb, &p->heavy_k, &p->heavy_shift, &p->pred, &p->decay};
-    if (int rc = launch(h, p->km->f_order, 1, 1024, 0, stream, b)) return rc;
-  }
+  int N = h->N, nslots = p->nblocks * p->wpb;
+  const int* stats = h->st.stats;
+  int* order = h->st.order;
+  void* b[] = {&N, &stats, &order, &p->slots, &nslots, &p->wpb, &p->pred};
+  if (int rc = launch(h, p->km->f_order, 1, 1024, 0, stream, b)) return rc;
   note_stream(p, stream);
   return 0;
 }

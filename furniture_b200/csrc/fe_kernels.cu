@@ -61,16 +61,19 @@ extern "C" __global__ void __launch_bounds__(32 * FE_MAX_WPB) fe_env_reset_kerne
 // the big Newton solve) bound the whole step by their own latency, which is lowest when few warps share the SM: they get
 // blocks with only `heavy_k` of the warp slots used, launched first, while the light envs fill the other SMs.
 #define FE_ORDER_BUCKETS 256
+#define FE_ORDER_HEAVY_SHIFT 18 /* heavy: 18 buckets above the median, 2^(18/16) = 2.2x the median work */
+#define FE_ORDER_HEAVY_K 7      /* warp slots used in a block of heavy envs (7 of 14); half the block where it holds fewer than 8 */
+#define FE_ORDER_DECAY 0.85f    /* per-step decay of an env's predicted work */
 extern "C" __global__ void __launch_bounds__(1024) fe_order_kernel(int N, const int* __restrict__ stats, int* __restrict__ order, int* __restrict__ slots, int nslots,
-                                                        int wpb, int heavy_k, int heavy_shift, float* __restrict__ pred, float decay) {
+                                                        int wpb, float* __restrict__ pred) {
   __shared__ int hist[FE_ORDER_BUCKETS], start[FE_ORDER_BUCKETS], nheavy;
-  const int tid = threadIdx.x;
+  const int tid = threadIdx.x, heavy_k = wpb > FE_ORDER_HEAVY_K ? FE_ORDER_HEAVY_K : wpb / 2;
   if (tid < FE_ORDER_BUCKETS) hist[tid] = 0;
   // predicted work of the next step: the last step's, but an env that was heavy a few steps ago is still suspect
   for (int e = tid; e < N; e += 1024) {
     const int* st = stats + (size_t)e * FE_NSTAT;
     const float work = (float)st[4] + (float)st[5] + (float)st[6] + (float)st[7] + (float)st[8]; // cycles / 16
-    pred[e] = fmaxf(work, decay * pred[e]);
+    pred[e] = fmaxf(work, FE_ORDER_DECAY * pred[e]);
   }
   __syncthreads();
   auto bucket_of = [&](int e) {
@@ -84,8 +87,8 @@ extern "C" __global__ void __launch_bounds__(1024) fe_order_kernel(int N, const 
   if (tid == 0) {
     int acc = 0, med = -1;
     for (int b = 0; b < FE_ORDER_BUCKETS; ++b) { start[b] = acc; acc += hist[b]; if (med < 0 && 2 * acc >= N) med = b; }
-    // heavy: at least heavy_shift buckets (sixteenths of an octave) above the median bucket
-    const int hb = med - heavy_shift; // last heavy bucket (buckets are in heaviest-first order)
+    // heavy: at least FE_ORDER_HEAVY_SHIFT buckets (sixteenths of an octave) above the median bucket
+    const int hb = med - FE_ORDER_HEAVY_SHIFT; // last heavy bucket (buckets are in heaviest-first order)
     const int H = (heavy_k > 0 && heavy_k < wpb && hb >= 0) ? start[hb] + hist[hb] : 0;
     const int cap = heavy_k * FE_EXTRA_BLOCKS;
     nheavy = H > cap ? cap : H;

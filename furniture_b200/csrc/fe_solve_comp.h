@@ -41,12 +41,7 @@ FE_FN void fe_solve_comp(FeWarp* w, int nA, int ncc, unsigned cplmask, int robot
   FE_PRIV(float, ox_); FE_PRIV(float, oy_); FE_PRIV(float, oz_); FE_PRIV(float, px_); FE_PRIV(float, py_); FE_PRIV(float, pz_);
   FE_PRIV(float, a_); FE_PRIV(float, b_); FE_PRIV(float, t_);
   FE_PRIV(int, any_);
-#if FE_DEVICE_BUILD
-#define COMP_TICK(slot) { long long t1_ = clock64(); if ((threadIdx.x & 31u) == 0) w->u()[slot] += (int)((t1_ - t0_) >> 4); t0_ = t1_; }
-  long long t0_ = clock64();
-#else
-#define COMP_TICK(slot)
-#endif
+  FE_TICK_START
 
   // ---------------------------------------------------------------- set-up (once per solve)
   int run = 0;
@@ -251,7 +246,7 @@ FE_FN void fe_solve_comp(FeWarp* w, int nA, int ncc, unsigned cplmask, int robot
   REGS_END                                                                                                                         \
   FE_WSUM(dst);
 
-  COMP_TICK(25)
+  FE_TICK(w->u(), 25)
   // ---- the two starting candidates: the unconstrained (smooth) acceleration and the warm start; the cheaper one is kept
   COMP_MULJ(w->as(), jv_, w->w_jv(), true)  // smooth candidate rows in jv_ / w_jv
   COMP_COST(jv_, w->w_jv(), as_, a_)
@@ -272,7 +267,7 @@ FE_FN void fe_solve_comp(FeWarp* w, int nA, int ncc, unsigned cplmask, int robot
     LANES_END
   }
 
-  COMP_TICK(26)
+  FE_TICK(w->u(), 26)
   // ---------------------------------------------------------------- Newton iterations
   int iter = 0;
   float impr = 0.f;
@@ -373,11 +368,8 @@ FE_FN void fe_solve_comp(FeWarp* w, int nA, int ncc, unsigned cplmask, int robot
       PV(b_) = g * g;
     LANES_END
     FE_WSUM(a_); FE_WSUM(b_);
-    COMP_TICK(27)
+    FE_TICK(w->u(), 27)
     const float cost = FE_UNI(a_), gnorm = sqrtf(FE_UNI(b_));
-#if !FE_DEVICE_BUILD
-    if (getenv("FE_DEBUG_SOLVE")) printf("  comp it %d nA %d ncc %d cost %.9g gnorm %.4g scaled-g %.3g impr %.3g\n", iter, nA, ncc, cost, gnorm, scale * gnorm, scale * impr);
-#endif
     if (!(cost == cost)) { LANES_BEGIN if (lane == 0) w->u()[2] |= 2; LANES_END break; }
     if (iter > 0) { if (scale * impr < tol || scale * gnorm < tol) break; }
     else if (scale * gnorm < tol) break;
@@ -466,7 +458,7 @@ FE_FN void fe_solve_comp(FeWarp* w, int nA, int ncc, unsigned cplmask, int robot
         }
       }
     }
-    COMP_TICK(28)
+    FE_TICK(w->u(), 28)
     // right-looking Cholesky, pivot column broadcast by shuffle
 #pragma unroll
     for (int k = 0; k < NMAX; ++k) {
@@ -506,14 +498,14 @@ FE_FN void fe_solve_comp(FeWarp* w, int nA, int ncc, unsigned cplmask, int robot
       if (PV(z_) >= 0) w->search()[PV(z_)] = PV(s_);
       if (PV(bad_) && lane == 0) w->u()[2] |= 4;
     LANES_END
-    COMP_TICK(29)
+    FE_TICK(w->u(), 29)
     // products with the search direction
     COMP_MULM(w->search(), Ms_)
     COMP_MULJ(w->search(), jv_, w->w_jv(), false)
     REGS_BEGIN PV(a_) = PV(s_) * PV(r_); PV(b_) = 0.5f * PV(s_) * PV(Ms_); REGS_END
     FE_WSUM(a_); FE_WSUM(b_);
     const float g1 = FE_UNI(a_), g2 = FE_UNI(b_);
-    COMP_TICK(30)
+    FE_TICK(w->u(), 30)
     // exact line search: safeguarded Newton on p'(alpha) = 0 (rtsafe rule: bisect unless the step at least halves)
     float p1 = 0.f, p2 = 0.f, lo = 0.f, hi = -1.f, alpha = 0.f, p1_0 = 0.f, dxold = 0.f;
     bool fail = false;
@@ -569,7 +561,7 @@ FE_FN void fe_solve_comp(FeWarp* w, int nA, int ncc, unsigned cplmask, int robot
       dxold = fabsf(next - alpha);
       alpha = next;
     }
-    COMP_TICK(31)
+    FE_TICK(w->u(), 31)
     if (fail || !(alpha > 0.f)) break;
     impr = -0.5f * alpha * p1_0;
     LANES_BEGIN
@@ -596,7 +588,6 @@ FE_FN void fe_solve_comp(FeWarp* w, int nA, int ncc, unsigned cplmask, int robot
     }
     if (lane == 0) { if (iter > w->u()[3]) w->u()[3] = iter; w->u()[7] += iter; w->u()[6] += 1; }
   LANES_END
-#undef COMP_TICK
 #undef COMP_MULJ
 #undef COMP_MULM
 #undef COMP_COST

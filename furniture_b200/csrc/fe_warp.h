@@ -41,6 +41,18 @@
 #define FE_BLOCK_SYNC ((void)0)
 #endif
 
+// Cycle counters of the per-call statistics: FE_TICK_START starts the clock in a function, FE_TICK(ctr, slot, ...) adds the
+// cycles since the previous tick (clock64 / 16, by lane 0) to ctr[slot] for every slot listed and restarts the clock.  The
+// emulated build has no clock: its counters stay 0.
+#if FE_DEVICE_BUILD
+#define FE_TICK_START long long t0_ = clock64();
+#define FE_TICK(ctr, ...) { const long long t1_ = clock64(); \
+    if ((threadIdx.x & 31u) == 0) { const int d_ = (int)((t1_ - t0_) >> 4), s_[] = {__VA_ARGS__}; for (int i_ : s_) (ctr)[i_] += d_; } t0_ = t1_; }
+#else
+#define FE_TICK_START
+#define FE_TICK(ctr, ...)
+#endif
+
 // sum of scr[0..31] with a fixed butterfly order (identical result on every lane and in the emulation build)
 FE_HD float fe_sum32(const float* scr) {
 #if FE_DEVICE_BUILD
