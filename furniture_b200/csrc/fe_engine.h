@@ -19,7 +19,10 @@
 #define FE_MINVAL 1e-15f
 #define FE_MINIMP 0.0001f
 #define FE_MAXIMP 0.9999f
-#define FE_MAXCAND 96
+// Broad-phase result in the slice: per lane, its 64-bit hit mask over its range of the pair list (two words) and the scan
+// offset of its first hit.  Any number of candidates fits; the narrow phase recovers candidate i from the owning lane's mask.
+#define FE_CAND_WORDS (3 * 32)
+static_assert(FE_MAXPAIR <= 32 * 64, "a broad-phase lane holds at most 64 pairs in its hit mask");
 // Line search: stop when |p'(alpha)| <= FE_LS_TOL |p'(0)|.  MuJoCo's default ls_tolerance is 0.01; the Newton loop's own
 // stopping test decides the final accuracy.  (1e-5 was below the fp32 noise of p' for a resting part: every line search of the
 // grouped part solver ran all 20 evaluations for bit-identical steps -- 20.0 passes per call against 4.0, measured on the
@@ -115,7 +118,7 @@ FE_BOTH int fe_layout_build(FeLayout* L, const fe_model* m, const FeOpt& opt) {
   L->Jc = L->lcrb; /* composite inertias (smooth stage) vs row staging of fe_build_H */
   CARVE(scr, 2 * 32) CARVE(first, nv) CARVE(skip, nv) CARVE(iscr, 32) CARVE(colmap, 32) CARVE(u, 4 + FE_NSTAT)
   // H (solver) and the collision scratch (geom poses, candidate list) are never live together: overlay them
-  const int hwords = fe_tri(nv), cwords = 12 * ng + FE_MAXCAND;
+  const int hwords = fe_tri(nv), cwords = 12 * ng + FE_CAND_WORDS;
   L->H = o; L->gpos = o; L->gmat = o + 3 * ng; L->cand = o + 12 * ng;
   o += hwords > cwords ? hwords : cwords;
 #undef CARVE
@@ -638,6 +641,26 @@ FE_HD int fe_lane_excl_scan(int n) {
 #define FE_SCAN(run, n) ((run += (n)), (run - (n)))
 #endif
 
+// position of the j-th set bit (from 0) of the 64-bit mask hi:lo; requires j < its population count
+FE_HD int fe_nth_bit(unsigned lo, unsigned hi, int j) {
+#if FE_DEVICE_BUILD
+#define FE_POPC(v) __popc(v)
+#else
+#define FE_POPC(v) __builtin_popcount(v)
+#endif
+  unsigned h = lo;
+  int pos = 0;
+  if (j >= FE_POPC(lo)) { j -= FE_POPC(lo); h = hi; pos = 32; }
+#pragma unroll
+  for (int s = 16; s >= 1; s >>= 1) {
+    const unsigned low = h & ((1u << s) - 1u);
+    const int c = FE_POPC(low);
+    if (j >= c) { j -= c; h >>= s; pos += s; } else h = low;
+  }
+#undef FE_POPC
+  return pos;
+}
+
 // A pair with a sensor geom (gap > 0; mj_collision reports its contacts, mj_makeConstraint skips those with dist >= margin - gap):
 // the contacts at or beyond `active` only raise the touch flags; the (rare) closer ones stay.  Returns the contacts kept.
 FE_HDN int fe_sensor_pair(FeWarp* w, int g1, int g2, FeCon* res, int n, float active) {
@@ -684,10 +707,11 @@ FE_FN void fe_collide(FeWarp* w) {
     }
     if (lane < m->npart) w->touch()[lane] = 0;
   LANES_END
-  // broad phase: every lane tests a contiguous range of the pair list (order preserved), one scan compacts the hits
+  // broad phase: every lane tests a contiguous range of the pair list (order preserved), one scan gives each lane the offset of
+  // its first hit in the candidate list
+  const int per = (npair + 31) / 32;
   int ncand = 0;
   {
-    const int per = (npair + 31) / 32;
     int run = 0;
     (void)run;
     LANES_BEGIN
@@ -716,15 +740,15 @@ FE_FN void fe_collide(FeWarp* w) {
 #else
       const int n = __builtin_popcountll(hits);
 #endif
-      int off = FE_SCAN(run, n);
-      for (int k = k0; k < k1; ++k)
-        if ((hits >> (k - k0)) & 1ull) { if (off < FE_MAXCAND) w->cand()[off] = k; ++off; }
-      if (lane == 31) w->iscr()[0] = off;
+      const int off = FE_SCAN(run, n);
+      w->cand()[lane] = (int)(unsigned)hits;
+      w->cand()[32 + lane] = (int)(unsigned)(hits >> 32);
+      w->cand()[64 + lane] = off;
+      if (lane == 31) w->iscr()[0] = off + n;
     LANES_END
     ncand = w->iscr()[0];
     LANES_BEGIN LANES_END
   }
-  if (ncand > FE_MAXCAND) { ncand = FE_MAXCAND; LANES_BEGIN if (lane == 0) w->u()[2] |= 1; LANES_END }
   int ncon = 0;
   for (int base = 0; base < ncand; base += 32) {
     int run = 0;
@@ -734,7 +758,12 @@ FE_FN void fe_collide(FeWarp* w) {
       FeCon res[8];
       int n = 0, g1 = 0, g2 = 0;
       if (ci < ncand) {
-        const int k = w->cand()[ci];
+        // candidate ci (pair-list order): owned by the last lane whose first hit is at or before ci -- a lane without hits shares
+        // its offset with the next lane, so the last such lane has hits -- and it is that lane's (ci - offset)-th hit
+        int o = 0;
+        for (int s = 16; s >= 1; s >>= 1)
+          if (w->cand()[64 + o + s] <= ci) o += s;
+        const int k = o * per + fe_nth_bit((unsigned)w->cand()[o], (unsigned)w->cand()[32 + o], ci - w->cand()[64 + o]);
         g1 = m->pair_g1[k]; g2 = m->pair_g2[k];
         const float mg = hasm ? fmaxf(m->geom_margin[g1], m->geom_margin[g2]) : 0.f;
         n = fe_narrowphase(m, g1, g2, w->gpos() + 3 * g1, w->gmat() + 9 * g1, w->gpos() + 3 * g2, w->gmat() + 9 * g2, mg, res);

@@ -184,9 +184,9 @@ def test_joint_limit_rows_match_oracle(sawyer_model, gpu):
 
 @pytest.mark.parametrize("gpu", BACKENDS)
 def test_grasped_part_coupled_solve_matches_oracle(sawyer_model, gpu):
-    """a leg pinched between the finger pads couples the robot block to a free part (FULL solver scope: cooperative Newton
-    with the register-resident direction for the coupled dofs, independent 6x6 blocks for the parts left on the floor):
-    constrained accelerations and a short trajectory follow the oracle."""
+    """a leg pinched between the finger pads couples the robot block to a free part (the coupled component of nA = 15 dofs,
+    solved by fe_solve_comp<16>; the parts left on the floor go to the grouped solver): constrained accelerations and a short
+    trajectory follow the oracle.  tests/test_solver_branches.py covers the other branches of fe_solve."""
     from oracle.ref_env import OracleFurnitureEnv
     from test_env_parity import _grasp_and_align_state
 
