@@ -291,22 +291,59 @@ FE_FN void fe_solve_blocks(FeWarp* w, const float* L, const int* skip, float* x)
   LANES_END
 }
 
+// Solves an SPD system held by rows in registers: lane i owns row i of the lower triangle in row_[0..NMAX) (rows and columns
+// beyond the system padded with the identity) and its right-hand side in b_, which holds x_i on exit.  Right-looking
+// Cholesky with the pivot column broadcast by shuffle, then y = L^-1 b and x = L^-T y (column k of L is spread over the
+// lanes: one butterfly sum per unknown).  bad_ is set where a pivot was not positive (it is replaced by 1e-30).
+#define FE_REG_CHOL_SOLVE(NMAX, row_, b_, bad_)                                                                                  \
+  {                                                                                                                                \
+    FE_PRIV(float, s0_); FE_PRIV(float, s1_); FE_PRIV(float, dinv_); FE_PRIV(float, q_);                                          \
+    REGS_BEGIN PV(bad_) = 0; PV(dinv_) = 1.f; REGS_END                                                                             \
+    _Pragma("unroll") for (int k = 0; k < (NMAX); ++k) {                                                                           \
+      FE_SHFLA(s0_, row_, k, k);                                                                                                   \
+      REGS_BEGIN                                                                                                                   \
+        float pk = PV(s0_);                                                                                                        \
+        if (!(pk > 1e-30f)) { PV(bad_) = 1; pk = 1e-30f; }                                                                         \
+        const float lkk = sqrtf(pk), inv = 1.0f / lkk;                                                                             \
+        const float lik = lane > k ? PV(row_)[k] * inv : (lane == k ? lkk : 0.f);                                                  \
+        PV(row_)[k] = lik;                                                                                                         \
+        PV(q_) = lik;                                                                                                              \
+        if (lane == k) PV(dinv_) = inv;                                                                                            \
+      REGS_END                                                                                                                     \
+      _Pragma("unroll") for (int j = k + 1; j < (NMAX); ++j) {                                                                     \
+        FE_SHFL(s1_, q_, j);                                                                                                       \
+        REGS_BEGIN PV(row_)[j] -= PV(q_) * PV(s1_); REGS_END                                                                       \
+      }                                                                                                                            \
+    }                                                                                                                              \
+    _Pragma("unroll") for (int k = 0; k < (NMAX); ++k) { /* y = L^-1 b */                                                         \
+      REGS_BEGIN PV(q_) = PV(b_) * PV(dinv_); REGS_END                                                                             \
+      FE_SHFL(s0_, q_, k);                                                                                                         \
+      REGS_BEGIN                                                                                                                   \
+        if (lane > k) PV(b_) -= PV(row_)[k] * PV(s0_);                                                                             \
+        else if (lane == k) PV(b_) = PV(s0_);                                                                                      \
+      REGS_END                                                                                                                     \
+    }                                                                                                                              \
+    _Pragma("unroll") for (int k = (NMAX) - 1; k >= 0; --k) { /* x = L^-T y */                                                    \
+      REGS_BEGIN PV(q_) = (lane > k && lane < (NMAX)) ? PV(row_)[k] * PV(b_) : 0.f; REGS_END                                       \
+      FE_WSUM(q_);                                                                                                                 \
+      REGS_BEGIN if (lane == k) PV(b_) = (PV(b_) - PV(q_)) * PV(dinv_); REGS_END                                                   \
+    }                                                                                                                              \
+  }
+
 // ---------------------------------------------------------------- kinematics + smooth dynamics
 // x = (Mr + hdamp * diag(dof_damping) + diag(dadd))^-1 b for the robot block (nr <= NMAX; dadd may be null): lane i owns row i of the lower triangle in
-// registers, the factorisation is right-looking with the pivot column broadcast by shuffle, the two triangular solves likewise
-// (the scheme of fe_newton_regs).  Two lane regions in all, against some forty for the cooperative slice version (a region per
-// column step of fe_chol and per unknown of fe_chol_solve): the smooth acceleration of fe_kin_smooth and the implicit-damping
+// registers, factored and solved by FE_REG_CHOL_SOLVE.  Two lane regions in all, against some forty for the cooperative
+// slice version (a region per column step of fe_chol and per unknown of fe_chol_solve): the smooth acceleration of
+// fe_kin_smooth and the implicit-damping
 // solve of fe_integrate were mostly barriers.  b and x may alias.  Rows and columns beyond nr are padded with the identity.
 template <int NMAX>
 FE_FN void fe_robot_solve_regs(FeWarp* w, float hdamp, const float* dadd, const float* b, float* x, int flagbit) {
   const fe_model* m = w->m;
   const int nr = m->nr;
   FE_PRIVA(float, row_, NMAX);
-  FE_PRIV(float, s0_); FE_PRIV(float, s1_); FE_PRIV(float, b_); FE_PRIV(float, dinv_); FE_PRIV(float, q_);
-  FE_PRIV(int, bad_);
+  FE_PRIV(float, b_); FE_PRIV(int, bad_);
   REGS_BEGIN
     const int i = lane;
-    PV(bad_) = 0; PV(dinv_) = 1.f;
 #pragma unroll
     for (int j = 0; j < NMAX; ++j) {
       float v = (j == i) ? 1.f : 0.f;
@@ -315,39 +352,7 @@ FE_FN void fe_robot_solve_regs(FeWarp* w, float hdamp, const float* dadd, const 
     }
     PV(b_) = i < nr ? b[i] : 0.f;
   REGS_END
-#pragma unroll
-  for (int k = 0; k < NMAX; ++k) {
-    FE_SHFLA(s0_, row_, k, k);
-    REGS_BEGIN
-      float pk = PV(s0_);
-      if (!(pk > 1e-30f)) { PV(bad_) = 1; pk = 1e-30f; }
-      const float lkk = sqrtf(pk), inv = 1.0f / lkk;
-      const float lik = lane > k ? PV(row_)[k] * inv : (lane == k ? lkk : 0.f);
-      PV(row_)[k] = lik;
-      PV(q_) = lik;
-      if (lane == k) PV(dinv_) = inv;
-    REGS_END
-#pragma unroll
-    for (int j = k + 1; j < NMAX; ++j) {
-      FE_SHFL(s1_, q_, j);
-      REGS_BEGIN PV(row_)[j] -= PV(q_) * PV(s1_); REGS_END
-    }
-  }
-#pragma unroll
-  for (int k = 0; k < NMAX; ++k) { // y = L^-1 b
-    REGS_BEGIN PV(q_) = PV(b_) * PV(dinv_); REGS_END
-    FE_SHFL(s0_, q_, k);
-    REGS_BEGIN
-      if (lane > k) PV(b_) -= PV(row_)[k] * PV(s0_);
-      else if (lane == k) PV(b_) = PV(s0_);
-    REGS_END
-  }
-#pragma unroll
-  for (int k = NMAX - 1; k >= 0; --k) { // x = L^-T y
-    REGS_BEGIN PV(q_) = (lane > k && lane < NMAX) ? PV(row_)[k] * PV(b_) : 0.f; REGS_END
-    FE_WSUM(q_);
-    REGS_BEGIN if (lane == k) PV(b_) = (PV(b_) - PV(q_)) * PV(dinv_); REGS_END
-  }
+  FE_REG_CHOL_SOLVE(NMAX, row_, b_, bad_)
   LANES_BEGIN
     if (lane < nr) x[lane] = PV(b_);
     if (PV(bad_) && lane == 0) w->u()[2] |= flagbit;
@@ -960,6 +965,111 @@ FE_FN void fe_assemble(FeWarp* w) {
 }
 
 // ---------------------------------------------------------------- solver pieces
+// Zone logic of one elliptic contact, inlined (outputs stay in registers): forces f, cost, and with WANTW the 3x3 weight
+// (xx yy zz xy xz yz); returns the state
+template <bool WANTW>
+FE_HD int fe_cone_t(float j0, float j1, float j2, float mu, float fr, float D0, float D1, float* f, float* cost, float* W) {
+  const float N = j0 * mu, U1 = j1 * fr, U2 = j2 * fr, T = sqrtf(U1 * U1 + U2 * U2);
+  if (N >= mu * T || (T <= 0.f && N >= 0.f)) { f[0] = f[1] = f[2] = 0.f; if (WANTW) { W[0] = W[1] = W[2] = W[3] = W[4] = W[5] = 0.f; } return 0; }
+  if (mu * N + T <= 0.f || (T <= 0.f && N < 0.f)) {
+    f[0] = -D0 * j0; f[1] = -D1 * j1; f[2] = -D1 * j2;
+    *cost += 0.5f * (D0 * j0 * j0 + D1 * (j1 * j1 + j2 * j2));
+    if (WANTW) { W[0] = D0; W[1] = D1; W[2] = D1; W[3] = W[4] = W[5] = 0.f; }
+    return 1;
+  }
+  const float Dm = D0 / (mu * mu * (1.f + mu * mu)), NmT = N - mu * T;
+  *cost += 0.5f * Dm * NmT * NmT;
+  f[0] = -Dm * NmT * mu;
+  f[1] = -f[0] / T * U1 * fr;
+  f[2] = -f[0] / T * U2 * fr;
+  if (WANTW) {
+    const float iT = 1.f / T, a = Dm * mu * mu * iT * iT, b = Dm * NmT * mu * iT;
+    const float h11 = a * U1 * U1 - b * (1.f - U1 * U1 * iT * iT), h22 = a * U2 * U2 - b * (1.f - U2 * U2 * iT * iT), h12 = a * U1 * U2 + b * U1 * U2 * iT * iT;
+    const float h01 = -Dm * mu * U1 * iT, h02 = -Dm * mu * U2 * iT;
+    W[0] = mu * mu * Dm; W[1] = fr * fr * h11; W[2] = fr * fr * h22; W[3] = mu * fr * h01; W[4] = mu * fr * h02; W[5] = fr * fr * h12;
+  }
+  return 2;
+}
+// One contact's terms of p'(alpha) and p''(alpha) along the search direction: rows j + alpha v, with v the rows of the
+// direction.  They are applied to d1 / d2 with `op` (= or +=) inside each zone; the zone without force leaves d1 / d2 alone.
+// A macro rather than a function that returns the terms: fe_line_eval's += then stays inside each zone's expression, as
+// the product it may be fused with, instead of becoming a separate add after the branch.
+#define FE_CONE_LS(j, v, alpha, mu_, fr_, D0_, D1_, d1, op, d2)                                                                    \
+  {                                                                                                                                \
+    const float *cj_ = (j), *cv_ = (v);                                                                                            \
+    const float al = (alpha), mu = (mu_), fr = (fr_), D0 = (D0_), D1 = (D1_);                                                      \
+    const float v0 = cv_[0], v1 = cv_[1], v2 = cv_[2];                                                                             \
+    const float x0 = cj_[0] + al * v0, x1 = cj_[1] + al * v1, x2 = cj_[2] + al * v2;                                               \
+    const float N = x0 * mu, U1 = x1 * fr, U2 = x2 * fr, T = sqrtf(U1 * U1 + U2 * U2);                                             \
+    if (N >= mu * T || (T <= 0.f && N >= 0.f)) {                                                                                   \
+    } else if (mu * N + T <= 0.f || (T <= 0.f && N < 0.f)) {                                                                       \
+      d1 op D0 * x0 * v0 + D1 * (x1 * v1 + x2 * v2);                                                                               \
+      d2 op D0 * v0 * v0 + D1 * (v1 * v1 + v2 * v2);                                                                               \
+    } else {                                                                                                                       \
+      const float Dm = D0 / (mu * mu * (1.f + mu * mu)), NmT = N - mu * T, N1 = v0 * mu, V1 = v1 * fr, V2 = v2 * fr;               \
+      const float T1 = (U1 * V1 + U2 * V2) / T, T2 = (V1 * V1 + V2 * V2 - T1 * T1) / T, a = N1 - mu * T1;                          \
+      d1 op Dm * NmT * a;                                                                                                          \
+      d2 op Dm * (a * a - NmT * mu * T2);                                                                                          \
+    }                                                                                                                              \
+  }
+
+// Exact line search along the Newton direction: safeguarded Newton on p'(alpha) = 0.  p' is only piecewise smooth (rows
+// change cone zone along the ray): a Newton step is kept only while it at least halves the previous one (rtsafe rule),
+// otherwise bisect -- else the iterates can hop between the two ends of the bracket and shrink it by almost nothing.
+// The caller evaluates p'(alpha), p''(alpha) and passes them to start() for the first evaluation (alpha = 0) and to step()
+// after that; both return false when the search is over.  alpha stays 0 when the direction is not a descent direction.
+struct FeLineSearch {
+  float alpha = 0.f, p1_0 = 0.f, lo = 0.f, hi = -1.f, dxold = 0.f;
+  FE_MEMBER bool start(float p1, float p2) {
+    if (!(p1 < 0.f) || !(p2 > 0.f)) return false;
+    p1_0 = p1;
+    alpha = -p1 / p2;
+    dxold = alpha;
+    return true;
+  }
+  FE_MEMBER bool step(float p1, float p2) {
+    if (fabsf(p1) <= FE_LS_TOL * fabsf(p1_0)) return false;
+    if (p1 < 0.f) lo = alpha; else hi = alpha;
+    float next = alpha - p1 / p2;
+    if (hi > 0.f && (!(next > lo && next < hi) || fabsf(2.f * p1) > fabsf(dxold * p2))) next = 0.5f * (lo + hi);
+    if (hi < 0.f && !(next > lo)) next = 2.f * alpha;
+    const bool more = !(fabsf(next - alpha) <= 1e-6f * fabsf(alpha)); // relative step below 1e-6: take it and stop
+    dxold = fabsf(next - alpha);
+    alpha = next;
+    return more;
+  }
+  // predicted decrease of the cost, -alpha p'(0) / 2 (exact for a quadratic): the improvement of the Newton stop test
+  FE_MEMBER float impr() const { return -0.5f * alpha * p1_0; }
+};
+// Newton stop test on the scaled improvement of the last step and the scaled gradient norm, then the iteration limit
+FE_HD bool fe_newton_stop(int iter, int maxit, float scale, float impr, float gnorm, float tol) {
+  if (iter > 0 ? (scale * impr < tol || scale * gnorm < tol) : scale * gnorm < tol) return true;
+  return iter >= maxit;
+}
+
+// Weld rows of weld e under the link accelerations staged in lacc2: v_A + w_A x r1 - v_B, then G (w_A - w_B)
+FE_HD void fe_weld_rows(const FeWarp* w, int e, float* r) {
+  const float *XA = w->lacc2() + 6 * w->m->eq_link1[e], *XB = w->lacc2() + 6 * w->m->eq_link2[e];
+  float t[3], dw[3];
+  v3cross(t, XA, w->w_r1() + 3 * e);
+  for (int k = 0; k < 3; ++k) r[k] = XA[3 + k] + t[k] - XB[3 + k];
+  v3sub(dw, XA, XB);
+  m3mulv(r + 3, w->w_G() + 9 * e, dw);
+}
+// Wr += the wrench of weld e's force w_f on link l (about the link's reference point), if l is one of its two links
+FE_HD void fe_weld_wrench(const FeWarp* w, int e, int l, float* Wr) {
+  const int A = w->m->eq_link1[e], B = w->m->eq_link2[e];
+  if (A != l && B != l) return;
+  const float* f = w->w_f() + 6 * e;
+  float tq[3], t[3];
+  m3tmulv(tq, w->w_G() + 9 * e, f + 3); // G^T f_rot
+  if (A == l) {
+    v3cross(t, w->w_r1() + 3 * e, f);
+    Wr[0] += t[0] + tq[0]; Wr[1] += t[1] + tq[1]; Wr[2] += t[2] + tq[2]; Wr[3] += f[0]; Wr[4] += f[1]; Wr[5] += f[2];
+  } else {
+    Wr[0] -= tq[0]; Wr[1] -= tq[1]; Wr[2] -= tq[2]; Wr[3] -= f[0]; Wr[4] -= f[1]; Wr[5] -= f[2];
+  }
+}
 // out = M_z in
 FE_FN void fe_mul_M(FeWarp* w, const float* in, float* out) {
   const fe_model* m = w->m;
@@ -1004,12 +1114,8 @@ FE_FN void fe_mul_J(FeWarp* w, const float* in, float* cout, float* wout, float*
     }
     for (int e = lane; e < ne; e += 32) {
       if (!w->eq_active()[e]) continue;
-      const float *XA = w->lacc2() + 6 * m->eq_link1[e], *XB = w->lacc2() + 6 * m->eq_link2[e];
-      float t[3], dw[3], r[6];
-      v3cross(t, XA, w->w_r1() + 3 * e);
-      for (int k = 0; k < 3; ++k) r[k] = XA[3 + k] + t[k] - XB[3 + k];
-      v3sub(dw, XA, XB);
-      m3mulv(r + 3, w->w_G() + 9 * e, dw);
+      float r[6];
+      fe_weld_rows(w, e, r);
       for (int k = 0; k < 6; ++k) wout[6 * e + k] = r[k] - (sub_aref ? w->w_aref()[6 * e + k] : 0.f);
     }
     for (int d = lane; d < nr; d += 32) lout[d] = w->l_sign()[d] * in[d] - (sub_aref ? w->l_aref()[d] : 0.f);
@@ -1024,25 +1130,9 @@ FE_FN float fe_update(FeWarp* w) {
     float cost = 0.f;
     for (int c = lane; c < ncon; c += 32) {
       if (fast && w->c_kind()[c] == 0) continue;
-      const float mu = w->c_mu()[c], fr = w->c_fric()[c], D0 = w->c_D()[2 * c], D1 = w->c_D()[2 * c + 1];
-      const float j0 = w->c_jar()[3 * c], j1 = w->c_jar()[3 * c + 1], j2 = w->c_jar()[3 * c + 2];
-      const float N = j0 * mu, U1 = j1 * fr, U2 = j2 * fr, T = sqrtf(U1 * U1 + U2 * U2);
-      float f0 = 0.f, f1 = 0.f, f2 = 0.f;
-      int st = 0;
-      if (N >= mu * T || (T <= 0.f && N >= 0.f)) st = 0;
-      else if (mu * N + T <= 0.f || (T <= 0.f && N < 0.f)) {
-        st = 1;
-        f0 = -D0 * j0; f1 = -D1 * j1; f2 = -D1 * j2;
-        cost += 0.5f * (D0 * j0 * j0 + D1 * (j1 * j1 + j2 * j2));
-      } else {
-        st = 2;
-        const float Dm = D0 / (mu * mu * (1.f + mu * mu)), NmT = N - mu * T;
-        cost += 0.5f * Dm * NmT * NmT;
-        f0 = -Dm * NmT * mu;
-        f1 = -f0 / T * U1 * fr;
-        f2 = -f0 / T * U2 * fr;
-      }
-      w->c_f()[3 * c] = f0; w->c_f()[3 * c + 1] = f1; w->c_f()[3 * c + 2] = f2;
+      float f[3];
+      const int st = fe_cone_t<false>(w->c_jar()[3 * c], w->c_jar()[3 * c + 1], w->c_jar()[3 * c + 2], w->c_mu()[c], w->c_fric()[c], w->c_D()[2 * c], w->c_D()[2 * c + 1], f, &cost, nullptr);
+      w->c_f()[3 * c] = f[0]; w->c_f()[3 * c + 1] = f[1]; w->c_f()[3 * c + 2] = f[2];
       w->c_state()[c] = st;
     }
     for (int e = lane; e < ne; e += 32) {
@@ -1088,20 +1178,8 @@ FE_FN void fe_mul_JT(FeWarp* w, float* out) {
         v3cross(t, r, fw);
         Wr[0] += sg * t[0]; Wr[1] += sg * t[1]; Wr[2] += sg * t[2]; Wr[3] += sg * fw[0]; Wr[4] += sg * fw[1]; Wr[5] += sg * fw[2];
       }
-      for (int e = 0; e < ne; ++e) {
-        if (!w->eq_active()[e]) continue;
-        const int A = m->eq_link1[e], B = m->eq_link2[e];
-        if (A != l && B != l) continue;
-        const float* f = w->w_f() + 6 * e;
-        float tq[3], t[3];
-        m3tmulv(tq, w->w_G() + 9 * e, f + 3); // G^T f_rot
-        if (A == l) {
-          v3cross(t, w->w_r1() + 3 * e, f);
-          Wr[0] += t[0] + tq[0]; Wr[1] += t[1] + tq[1]; Wr[2] += t[2] + tq[2]; Wr[3] += f[0]; Wr[4] += f[1]; Wr[5] += f[2];
-        } else {
-          Wr[0] -= tq[0]; Wr[1] -= tq[1]; Wr[2] -= tq[2]; Wr[3] -= f[0]; Wr[4] -= f[1]; Wr[5] -= f[2];
-        }
-      }
+      for (int e = 0; e < ne; ++e)
+        if (w->eq_active()[e]) fe_weld_wrench(w, e, l, Wr);
       for (int k = 0; k < 6; ++k) w->lacc2()[6 * l + k] = Wr[k];
       if (l >= nrl) for (int k = 0; k < 6; ++k) out[nr + 6 * (l - nrl) + k] = Wr[k];
     }
@@ -1125,21 +1203,7 @@ FE_FN void fe_line_eval(FeWarp* w, float alpha, float g1, float g2, float* d1, f
     float p1 = 0.f, p2 = 0.f;
     for (int c = lane; c < ncon; c += 32) {
       if (fast && w->c_kind()[c] == 0) continue;
-      const float mu = w->c_mu()[c], fr = w->c_fric()[c], D0 = w->c_D()[2 * c], D1 = w->c_D()[2 * c + 1];
-      const float v0 = w->c_jv()[3 * c], v1 = w->c_jv()[3 * c + 1], v2 = w->c_jv()[3 * c + 2];
-      const float x0 = w->c_jar()[3 * c] + alpha * v0, x1 = w->c_jar()[3 * c + 1] + alpha * v1, x2 = w->c_jar()[3 * c + 2] + alpha * v2;
-      const float N = x0 * mu, U1 = x1 * fr, U2 = x2 * fr, T = sqrtf(U1 * U1 + U2 * U2);
-      if (N >= mu * T || (T <= 0.f && N >= 0.f)) {
-      } else if (mu * N + T <= 0.f || (T <= 0.f && N < 0.f)) {
-        p1 += D0 * x0 * v0 + D1 * (x1 * v1 + x2 * v2);
-        p2 += D0 * v0 * v0 + D1 * (v1 * v1 + v2 * v2);
-      } else {
-        const float Dm = D0 / (mu * mu * (1.f + mu * mu)), NmT = N - mu * T;
-        const float N1 = v0 * mu, V1 = v1 * fr, V2 = v2 * fr;
-        const float T1 = (U1 * V1 + U2 * V2) / T, T2 = (V1 * V1 + V2 * V2 - T1 * T1) / T, a = N1 - mu * T1;
-        p1 += Dm * NmT * a;
-        p2 += Dm * (a * a - NmT * mu * T2);
-      }
+      FE_CONE_LS(w->c_jar() + 3 * c, w->c_jv() + 3 * c, alpha, w->c_mu()[c], w->c_fric()[c], w->c_D()[2 * c], w->c_D()[2 * c + 1], p1, +=, p2)
     }
     for (int e = lane; e < ne; e += 32) {
       if (!w->eq_active()[e]) continue;
@@ -1159,53 +1223,6 @@ FE_FN void fe_line_eval(FeWarp* w, float alpha, float g1, float g2, float* d1, f
   *d2 = fe_sum32(w->scr() + 32) + 2.f * g2;
 }
 
-// fe_cone, inlined (outputs stay in registers): zone, force, cost, and with WANTW the 3x3 weight (xx yy zz xy xz yz)
-template <bool WANTW>
-FE_HD int fe_cone_t(float j0, float j1, float j2, float mu, float fr, float D0, float D1, float* f, float* cost, float* W) {
-  const float N = j0 * mu, U1 = j1 * fr, U2 = j2 * fr, T = sqrtf(U1 * U1 + U2 * U2);
-  if (N >= mu * T || (T <= 0.f && N >= 0.f)) { f[0] = f[1] = f[2] = 0.f; if (WANTW) { W[0] = W[1] = W[2] = W[3] = W[4] = W[5] = 0.f; } return 0; }
-  if (mu * N + T <= 0.f || (T <= 0.f && N < 0.f)) {
-    f[0] = -D0 * j0; f[1] = -D1 * j1; f[2] = -D1 * j2;
-    *cost += 0.5f * (D0 * j0 * j0 + D1 * (j1 * j1 + j2 * j2));
-    if (WANTW) { W[0] = D0; W[1] = D1; W[2] = D1; W[3] = W[4] = W[5] = 0.f; }
-    return 1;
-  }
-  const float Dm = D0 / (mu * mu * (1.f + mu * mu)), NmT = N - mu * T;
-  *cost += 0.5f * Dm * NmT * NmT;
-  f[0] = -Dm * NmT * mu;
-  f[1] = -f[0] / T * U1 * fr;
-  f[2] = -f[0] / T * U2 * fr;
-  if (WANTW) {
-    const float iT = 1.f / T, a = Dm * mu * mu * iT * iT, b = Dm * NmT * mu * iT;
-    const float h11 = a * U1 * U1 - b * (1.f - U1 * U1 * iT * iT), h22 = a * U2 * U2 - b * (1.f - U2 * U2 * iT * iT), h12 = a * U1 * U2 + b * U1 * U2 * iT * iT;
-    const float h01 = -Dm * mu * U1 * iT, h02 = -Dm * mu * U2 * iT;
-    W[0] = mu * mu * Dm; W[1] = fr * fr * h11; W[2] = fr * fr * h22; W[3] = mu * fr * h01; W[4] = mu * fr * h02; W[5] = fr * fr * h12;
-  }
-  return 2;
-}
-// zone logic of one elliptic contact: forces f, cost, and (if W) the 3x3 weight (xx yy zz xy xz yz); returns state
-FE_HDN int fe_cone(float j0, float j1, float j2, float mu, float fr, float D0, float D1, float* f, float* cost, float* W) {
-  const float N = j0 * mu, U1 = j1 * fr, U2 = j2 * fr, T = sqrtf(U1 * U1 + U2 * U2);
-  if (N >= mu * T || (T <= 0.f && N >= 0.f)) { f[0] = f[1] = f[2] = 0.f; return 0; }
-  if (mu * N + T <= 0.f || (T <= 0.f && N < 0.f)) {
-    f[0] = -D0 * j0; f[1] = -D1 * j1; f[2] = -D1 * j2;
-    *cost += 0.5f * (D0 * j0 * j0 + D1 * (j1 * j1 + j2 * j2));
-    if (W) { W[0] = D0; W[1] = D1; W[2] = D1; W[3] = W[4] = W[5] = 0.f; }
-    return 1;
-  }
-  const float Dm = D0 / (mu * mu * (1.f + mu * mu)), NmT = N - mu * T;
-  *cost += 0.5f * Dm * NmT * NmT;
-  f[0] = -Dm * NmT * mu;
-  f[1] = -f[0] / T * U1 * fr;
-  f[2] = -f[0] / T * U2 * fr;
-  if (W) {
-    const float iT = 1.f / T, a = Dm * mu * mu * iT * iT, b = Dm * NmT * mu * iT;
-    const float h11 = a * U1 * U1 - b * (1.f - U1 * U1 * iT * iT), h22 = a * U2 * U2 - b * (1.f - U2 * U2 * iT * iT), h12 = a * U1 * U2 + b * U1 * U2 * iT * iT;
-    const float h01 = -Dm * mu * U1 * iT, h02 = -Dm * mu * U2 * iT;
-    W[0] = mu * mu * Dm; W[1] = fr * fr * h11; W[2] = fr * fr * h22; W[3] = mu * fr * h01; W[4] = mu * fr * h02; W[5] = fr * fr * h12;
-  }
-  return 2;
-}
 // rows of one part-vs-world contact in the part's coordinates: J[k] = sgn * [(r x F_k), F_k], r = pos - origin
 FE_HD void fe_part_rows(const FeWarp* w, int c, int l, float sgn, float* J) {
   float F[9];
@@ -1236,38 +1253,41 @@ FE_HD void fe_contact_weight(const FeWarp* w, int c, int st, float* W) {
     for (int a = 0; a < 3; ++a) for (int b = 0; b < 3; ++b) W[3 * a + b] = sc[a] * HU[3 * a + b] * sc[b];
   }
 }
-// column z of the 3-row contact Jacobian (contact frame; B side minus A side), z in solver coordinates
-FE_HD void fe_contact_col(const FeWarp* w, int c, int z, int A, int B, float* col) {
-  const fe_model* m = w->m;
-  const int nr = m->nr, nrl = m->nrlink;
-  float F[9];
-      fe_frame_load(w, c, F);
-  const float* p = w->c_pos() + 3 * c;
-  col[0] = col[1] = col[2] = 0.f;
-  if (z < 0) return;
-  if (z < nr) {
-    const float sg = ((B >= 0 && B < nrl && ((m->link_ancmask[B] >> z) & 1)) ? 1.f : 0.f) - ((A >= 0 && A < nrl && ((m->link_ancmask[A] >> z) & 1)) ? 1.f : 0.f);
+// twist [angular; linear at p0] that a unit of dof z (solver coordinates) gives the link pair (A, B), B side minus A side.
+// mA / mB are the robot ancestor masks of A / B (0 for a part or the world).
+FE_HD void fe_unit_twist(const FeWarp* w, int z, int A, int B, int mA, int mB, const float* p0, const float* Pr, float* d) {
+  const int nr = w->m->nr, nrl = w->m->nrlink;
+#pragma unroll
+  for (int q = 0; q < 6; ++q) d[q] = 0.f;
+  if (z >= 0 && z < nr) {
+    const float sg = (float)((mB >> z) & 1) - (float)((mA >> z) & 1);
     if (sg != 0.f) {
-      float r[3], t[3], v[3];
-      v3sub(r, p, m->robot_ref);
-      v3cross(t, w->S() + 6 * z, r);
-      v3add(v, w->S() + 6 * z + 3, t);
-      for (int k = 0; k < 3; ++k) col[k] = sg * v3dot(F + 3 * k, v);
+      const float* S = w->S() + 6 * z;
+      const float r[3] = {p0[0] - Pr[0], p0[1] - Pr[1], p0[2] - Pr[2]};
+      float t[3];
+      v3cross(t, S, r);
+      d[0] = sg * S[0]; d[1] = sg * S[1]; d[2] = sg * S[2]; d[3] = sg * (S[3] + t[0]); d[4] = sg * (S[4] + t[1]); d[5] = sg * (S[5] + t[2]);
     }
-  } else {
+  } else if (z >= nr) {
     const int part = (z - nr) / 6, jj = (z - nr) % 6, l = nrl + part;
     const float sg = l == B ? 1.f : (l == A ? -1.f : 0.f);
     if (sg != 0.f) {
-      float r[3];
-      v3sub(r, p, w->lpos() + 3 * l);
-      for (int k = 0; k < 3; ++k) {
-        if (jj < 3) { float t[3]; v3cross(t, r, F + 3 * k); col[k] = sg * (jj == 0 ? t[0] : (jj == 1 ? t[1] : t[2])); }
-        else col[k] = sg * (jj == 3 ? F[3 * k] : (jj == 4 ? F[3 * k + 1] : F[3 * k + 2])); // selects keep F in registers
-      }
+      if (jj < 3) {
+        const float e[3] = {jj == 0 ? 1.f : 0.f, jj == 1 ? 1.f : 0.f, jj == 2 ? 1.f : 0.f};
+        const float r[3] = {p0[0] - w->lpos()[3 * l], p0[1] - w->lpos()[3 * l + 1], p0[2] - w->lpos()[3 * l + 2]};
+        float t[3];
+        v3cross(t, e, r);
+        d[0] = sg * e[0]; d[1] = sg * e[1]; d[2] = sg * e[2]; d[3] = sg * t[0]; d[4] = sg * t[1]; d[5] = sg * t[2];
+      } else { d[3] = jj == 3 ? sg : 0.f; d[4] = jj == 4 ? sg : 0.f; d[5] = jj == 5 ? sg : 0.f; } // selects keep d in registers
     }
   }
 }
 
+// fe_cone_t<true> behind a call, for fe_build_H's grouped block: inlined there it changes the last bits of the
+// cooperative solver's results on sm_90a, so it stays out of line as it always was
+FE_HDN int fe_cone(float j0, float j1, float j2, float mu, float fr, float D0, float D1, float* f, float* cost, float* W) {
+  return fe_cone_t<true>(j0, j1, j2, mu, fr, D0, D1, f, cost, W);
+}
 // H = M_z + J^T W J  (packed lower, skyline first[]).  With regs set, the contacts that couple moving blocks are left to
 // fe_newton_regs (they are added to the register-resident rows there).
 FE_FN void fe_build_H(FeWarp* w, bool regs = false) {
@@ -1465,18 +1485,17 @@ FE_FN void fe_build_H(FeWarp* w, bool regs = false) {
 
 // Newton direction of the active dofs (robot + coupled parts, at most 32): lane i owns row i of the lower triangle of H in
 // registers.  Rows start from the slice copy (M_z, static-world contacts of the parts, welds, limits); the contacts that
-// couple blocks are added as rank-3 updates whose columns travel by shuffle; the factorisation is right-looking
-// (pivot column broadcast by shuffle), the two triangular solves likewise.  No slice traffic, no barriers inside.
+// couple blocks are added as rank-6 updates whose columns travel by shuffle; FE_REG_CHOL_SOLVE factors and solves.  No slice
+// traffic, no barriers inside.
 // NMAX (16 / 24 / 32) bounds the unrolled loops; rows and columns beyond nA are padded with the identity.
 template <int NMAX>
 FE_FN void fe_newton_regs(FeWarp* w, int nA) {
   const int ncon = w->u()[0];
   FE_PRIVA(float, row_, NMAX);
-  FE_PRIV(float, s0_); FE_PRIV(float, s1_); FE_PRIV(float, b_); FE_PRIV(float, dinv_); FE_PRIV(float, q_);
-  FE_PRIV(int, z_); FE_PRIV(int, bad_);
+  FE_PRIV(float, b_); FE_PRIV(int, z_); FE_PRIV(int, bad_);
   REGS_BEGIN
     const int i = lane, zi = i < nA ? w->colmap()[i] : -1;
-    PV(z_) = zi; PV(bad_) = 0; PV(dinv_) = 1.f;
+    PV(z_) = zi;
     const int fi = zi >= 0 ? w->first()[zi] : 0;
     const float* Hi = w->H() + fe_tri(zi >= 0 ? zi : 0);
 #pragma unroll
@@ -1494,7 +1513,7 @@ FE_FN void fe_newton_regs(FeWarp* w, int nA) {
   // entry of K, then a rank-6 update of the rows (6 shuffles per column) instead of a rank-3 update per contact.
   {
     const fe_model* m = w->m;
-    const int nr = m->nr, nrl = m->nrlink;
+    const int nrl = m->nrlink;
     FE_PRIVA(float, kq_, 21);
     FE_PRIVA(float, d_, 6); FE_PRIVA(float, u_, 6);
     FE_PRIV(float, px_); FE_PRIV(float, py_); FE_PRIV(float, pz_); FE_PRIV(float, ox_); FE_PRIV(float, oy_); FE_PRIV(float, oz_);
@@ -1549,35 +1568,10 @@ FE_FN void fe_newton_regs(FeWarp* w, int nA) {
         REGS_BEGIN PV(kf_) = (float)PV(key_); REGS_END // link ids fit a float exactly (two bytes)
         FE_SHFL(ks_, PV_ALL(kf_), g);
         const int gkey = (int)FE_UNI(ks_), A = (gkey & 255) - 1, B = (gkey >> 8) - 1;
+        const int mA = (A >= 0 && A < nrl) ? m->link_ancmask[A] : 0, mB = (B >= 0 && B < nrl) ? m->link_ancmask[B] : 0;
+        const float p0[3] = {p0x, p0y, p0z};
         // this lane's dof: its unit contribution to the relative twist of the pair, at p0
-        REGS_BEGIN
-          const int z = PV(z_);
-          float d[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-          if (z >= 0 && z < nr) {
-            const float sg = ((B >= 0 && B < nrl && ((m->link_ancmask[B] >> z) & 1)) ? 1.f : 0.f) - ((A >= 0 && A < nrl && ((m->link_ancmask[A] >> z) & 1)) ? 1.f : 0.f);
-            if (sg != 0.f) {
-              const float* S = w->S() + 6 * z;
-              const float r[3] = {p0x - m->robot_ref[0], p0y - m->robot_ref[1], p0z - m->robot_ref[2]};
-              float t[3];
-              v3cross(t, S, r);
-              d[0] = sg * S[0]; d[1] = sg * S[1]; d[2] = sg * S[2]; d[3] = sg * (S[3] + t[0]); d[4] = sg * (S[4] + t[1]); d[5] = sg * (S[5] + t[2]);
-            }
-          } else if (z >= nr) {
-            const int part = (z - nr) / 6, jj = (z - nr) % 6, l = nrl + part;
-            const float sg = l == B ? 1.f : (l == A ? -1.f : 0.f);
-            if (sg != 0.f) {
-              if (jj < 3) {
-                const float e[3] = {jj == 0 ? 1.f : 0.f, jj == 1 ? 1.f : 0.f, jj == 2 ? 1.f : 0.f};
-                const float r[3] = {p0x - w->lpos()[3 * l], p0y - w->lpos()[3 * l + 1], p0z - w->lpos()[3 * l + 2]};
-                float t[3];
-                v3cross(t, e, r);
-                d[0] = sg * e[0]; d[1] = sg * e[1]; d[2] = sg * e[2]; d[3] = sg * t[0]; d[4] = sg * t[1]; d[5] = sg * t[2];
-              } else d[jj] = sg;
-            }
-          }
-#pragma unroll
-          for (int k = 0; k < 6; ++k) PV(d_)[k] = d[k];
-        REGS_END
+        REGS_BEGIN fe_unit_twist(w, PV(z_), A, B, mA, mB, p0, m->robot_ref, PV(d_)); REGS_END
         // K d_i: entry by entry, K[a][b] = warp sum of the members' terms
 #pragma unroll
         for (int k = 0; k < 6; ++k) { REGS_BEGIN PV(u_)[k] = 0.f; REGS_END }
@@ -1605,42 +1599,7 @@ FE_FN void fe_newton_regs(FeWarp* w, int nA) {
       }
     }
   }
-  // right-looking Cholesky
-#pragma unroll
-  for (int k = 0; k < NMAX; ++k) {
-    FE_SHFLA(s0_, row_, k, k);
-    REGS_BEGIN
-      float pk = PV(s0_);
-      if (!(pk > 1e-30f)) { PV(bad_) = 1; pk = 1e-30f; }
-      const float lkk = sqrtf(pk), inv = 1.0f / lkk;
-      const float lik = lane > k ? PV(row_)[k] * inv : (lane == k ? lkk : 0.f);
-      PV(row_)[k] = lik;
-      PV(q_) = lik;
-      if (lane == k) PV(dinv_) = inv;
-    REGS_END
-#pragma unroll
-    for (int j = k + 1; j < NMAX; ++j) {
-      FE_SHFL(s1_, q_, j);
-      REGS_BEGIN PV(row_)[j] -= PV(q_) * PV(s1_); REGS_END
-    }
-  }
-  // forward substitution: y = L^-1 b
-#pragma unroll
-  for (int k = 0; k < NMAX; ++k) {
-    REGS_BEGIN PV(q_) = PV(b_) * PV(dinv_); REGS_END
-    FE_SHFL(s0_, q_, k);
-    REGS_BEGIN
-      if (lane > k) PV(b_) -= PV(row_)[k] * PV(s0_);
-      else if (lane == k) PV(b_) = PV(s0_);
-    REGS_END
-  }
-  // backward substitution: x = L^-T y (column k of L is spread over the lanes: one butterfly sum per unknown)
-#pragma unroll
-  for (int k = NMAX - 1; k >= 0; --k) {
-    REGS_BEGIN PV(q_) = (lane > k && lane < NMAX) ? PV(row_)[k] * PV(b_) : 0.f; REGS_END
-    FE_WSUM(q_);
-    REGS_BEGIN if (lane == k) PV(b_) = (PV(b_) - PV(q_)) * PV(dinv_); REGS_END
-  }
+  FE_REG_CHOL_SOLVE(NMAX, row_, b_, bad_)
   LANES_BEGIN
     if (PV(z_) >= 0) w->search()[PV(z_)] = PV(b_);
     if (PV(bad_) && lane == 0) w->u()[2] |= 4;
@@ -1750,9 +1709,7 @@ FE_FN void fe_solve_coop(FeWarp* w) {
     if (!(cost == cost)) { LANES_BEGIN if (lane == 0) w->u()[2] |= 2; LANES_END break; }
     // MuJoCo stops on scale*(oldcost - cost) < tol; in fp32 that difference of two large costs is round-off, so the
     // improvement is taken from the line search instead: -alpha p'(0) / 2 (exact for a quadratic, the Newton decrement)
-    if (iter > 0) { if (scale * impr < w->opt.tolerance || scale * gnorm < w->opt.tolerance) break; }
-    else if (scale * gnorm < w->opt.tolerance) break;
-    if (iter >= w->opt.newton_iters) break;
+    if (fe_newton_stop(iter, w->opt.newton_iters, scale, impr, gnorm, w->opt.tolerance)) break;
     FE_TICK(w->u(), 27)
     fe_build_H(w, regs);
     FE_TICK(w->u(), 28)
@@ -1783,30 +1740,18 @@ FE_FN void fe_solve_coop(FeWarp* w) {
       w->scr()[lane] = a; w->scr()[32 + lane] = b;
     LANES_END
     const float g1 = fe_sum32(w->scr()), g2 = fe_sum32(w->scr() + 32);
-    // exact line search: safeguarded Newton on p'(alpha) = 0
-    float p1, p2, lo = 0.f, hi = -1.f, alpha;
+    FeLineSearch ls;
+    float p1, p2;
     fe_line_eval(w, 0.f, g1, g2, &p1, &p2);
-    if (!(p1 < 0.f) || !(p2 > 0.f)) break;
-    const float p1_0 = p1;
-    alpha = -p1 / p2;
-    // p' is only piecewise smooth (rows change cone zone along the ray): a Newton step is kept only while it at least
-    // halves the previous one (rtsafe rule), otherwise bisect -- else the iterates can hop between the two ends of the
-    // bracket and shrink it by almost nothing
-    float dxold = alpha;
-    for (int ls = 0; ls < w->opt.ls_iters; ++ls) {
-      fe_line_eval(w, alpha, g1, g2, &p1, &p2);
-      if (fabsf(p1) <= FE_LS_TOL * fabsf(p1_0)) break;
-      if (p1 < 0.f) lo = alpha; else hi = alpha;
-      float next = alpha - p1 / p2;
-      if (hi > 0.f && (!(next > lo && next < hi) || fabsf(2.f * p1) > fabsf(dxold * p2))) next = 0.5f * (lo + hi);
-      if (hi < 0.f && !(next > lo)) next = 2.f * alpha;
-      if (fabsf(next - alpha) <= 1e-6f * fabsf(alpha)) { alpha = next; break; }
-      dxold = fabsf(next - alpha);
-      alpha = next;
+    if (!ls.start(p1, p2)) break;
+    for (int k = 0; k < w->opt.ls_iters; ++k) {
+      fe_line_eval(w, ls.alpha, g1, g2, &p1, &p2);
+      if (!ls.step(p1, p2)) break;
     }
     FE_TICK(w->u(), 31)
+    const float alpha = ls.alpha;
     if (!(alpha > 0.f)) break;
-    impr = -0.5f * alpha * p1_0;
+    impr = ls.impr();
     LANES_BEGIN
       for (int i = lane; i < nv; i += 32) { w->x()[i] += alpha * w->search()[i]; w->Ma()[i] += alpha * w->Mv()[i]; }
       for (int c = lane; c < ncon; c += 32) {
@@ -1851,8 +1796,7 @@ FE_FN void fe_solve_parts_grouped(FeWarp* w, unsigned skipmask) {
     FE_PRIVA(float, J_, 18); FE_PRIVA(float, par_, 4); // par_: D0, D1, mu, friction scale
     FE_PRIVA(float, x_, 6);
     FE_PRIVA(float, acc_, 28); FE_PRIVA(float, sd_, 6); FE_PRIVA(float, jx_, 3); FE_PRIVA(float, jv_, 3);
-    FE_PRIV(float, scale_); FE_PRIV(float, impr_); FE_PRIV(float, g1_); FE_PRIV(float, g2_); FE_PRIV(float, alpha_);
-    FE_PRIV(float, lo_); FE_PRIV(float, hi_); FE_PRIV(float, p10_); FE_PRIV(float, dx_);
+    FE_PRIV(float, scale_); FE_PRIV(float, impr_); FE_PRIV(float, g1_); FE_PRIV(float, g2_); FE_PRIV(FeLineSearch, ls_);
     LANES_BEGIN
       int part = np, slot = 0;
       PV(wide_) = 0; PV(lead_) = 0;
@@ -1950,11 +1894,9 @@ FE_FN void fe_solve_parts_grouped(FeWarp* w, unsigned skipmask) {
           fe_inert_sym6_add(H, I);
           for (int k = 0; k < 6; ++k) { Mx[k] -= w->fs()[z + k]; g[k] = Mx[k] + PV(acc_)[k]; gsq += g[k] * g[k]; }
           const float gnorm = sqrtf(gsq);
-          bool stop = false;
-          if (!(gnorm == gnorm)) { stop = true; if (PV(lead_)) w->u()[2] |= 2; }
-          else if (PV(iter_) > 0) stop = PV(scale_) * PV(impr_) < tol || PV(scale_) * gnorm < tol;
-          else stop = PV(scale_) * gnorm < tol;
-          if (PV(iter_) >= maxit) stop = true;
+          bool stop = true;
+          if (!(gnorm == gnorm)) { if (PV(lead_)) w->u()[2] |= 2; }
+          else stop = fe_newton_stop(PV(iter_), maxit, PV(scale_), PV(impr_), gnorm, tol);
           if (stop) PV(act_) = 0;
           else {
             if (!fe_chol6(H) && PV(lead_)) w->u()[2] |= 4;
@@ -1963,7 +1905,7 @@ FE_FN void fe_solve_parts_grouped(FeWarp* w, unsigned skipmask) {
             float Ms[6], g1 = 0.f, g2 = 0.f;
             inert_mulv(Ms, I, PV(sd_));
             for (int k = 0; k < 6; ++k) { g1 += PV(sd_)[k] * Mx[k]; g2 += 0.5f * PV(sd_)[k] * Ms[k]; }
-            PV(g1_) = g1; PV(g2_) = g2; PV(alpha_) = 0.f; PV(lo_) = 0.f; PV(hi_) = -1.f; PV(dx_) = 0.f; PV(lsact_) = 1;
+            PV(g1_) = g1; PV(g2_) = g2; PV(ls_) = FeLineSearch(); PV(lsact_) = 1;
             if (PV(c_) >= 0) {
               const float* J = PV(J_);
               for (int k = 0; k < 3; ++k) PV(jv_)[k] = dot6(J + 6 * k, PV(sd_));
@@ -1979,50 +1921,25 @@ FE_FN void fe_solve_parts_grouped(FeWarp* w, unsigned skipmask) {
           float p1 = 0.f, p2 = 0.f;
           if (PV(lsact_) && PV(c_) >= 0) {
             const float* q = PV(par_);
-            const float al = PV(alpha_), mu = q[2], fr = q[3], D0 = q[0], D1 = q[1];
-            const float v0 = PV(jv_)[0], v1 = PV(jv_)[1], v2 = PV(jv_)[2];
-            const float x0 = PV(jx_)[0] + al * v0, x1 = PV(jx_)[1] + al * v1, x2 = PV(jx_)[2] + al * v2;
-            const float N = x0 * mu, U1 = x1 * fr, U2 = x2 * fr, T = sqrtf(U1 * U1 + U2 * U2);
-            if (N >= mu * T || (T <= 0.f && N >= 0.f)) {
-            } else if (mu * N + T <= 0.f || (T <= 0.f && N < 0.f)) {
-              p1 = D0 * x0 * v0 + D1 * (x1 * v1 + x2 * v2);
-              p2 = D0 * v0 * v0 + D1 * (v1 * v1 + v2 * v2);
-            } else {
-              const float Dm = D0 / (mu * mu * (1.f + mu * mu)), NmT = N - mu * T, N1 = v0 * mu, V1 = v1 * fr, V2 = v2 * fr;
-              const float T1 = (U1 * V1 + U2 * V2) / T, T2 = (V1 * V1 + V2 * V2 - T1 * T1) / T, a = N1 - mu * T1;
-              p1 = Dm * NmT * a;
-              p2 = Dm * (a * a - NmT * mu * T2);
-            }
+            FE_CONE_LS(PV(jx_), PV(jv_), PV(ls_).alpha, q[2], q[3], q[0], q[1], p1, =, p2)
           }
           PV(acc_)[0] = p1; PV(acc_)[1] = p2;
         LANES_END
         FE_GSUMV_ARRN(acc_, 28, 2, PV_ALL(wide_));
         LANES_BEGIN
           if (PV(lsact_)) {
-            const float al = PV(alpha_);
+            const float al = PV(ls_).alpha;
             const float p1 = PV(acc_)[0] + PV(g1_) + 2.f * al * PV(g2_), p2 = PV(acc_)[1] + 2.f * PV(g2_);
-            if (ls == 0) {
-              if (!(p1 < 0.f) || !(p2 > 0.f)) { PV(lsact_) = 0; PV(act_) = 0; PV(alpha_) = 0.f; }
-              else { PV(p10_) = p1; PV(alpha_) = -p1 / p2; PV(dx_) = PV(alpha_); }
-            } else if (fabsf(p1) <= FE_LS_TOL * fabsf(PV(p10_))) PV(lsact_) = 0;
-            else {
-              if (p1 < 0.f) PV(lo_) = al; else PV(hi_) = al;
-              float next = al - p1 / p2;
-              if (PV(hi_) > 0.f && (!(next > PV(lo_) && next < PV(hi_)) || fabsf(2.f * p1) > fabsf(PV(dx_) * p2))) next = 0.5f * (PV(lo_) + PV(hi_)); // rtsafe rule
-              if (PV(hi_) < 0.f && !(next > PV(lo_))) next = 2.f * al;
-              if (fabsf(next - al) <= 1e-6f * fabsf(al)) PV(lsact_) = 0;
-              PV(dx_) = fabsf(next - al);
-              PV(alpha_) = next;
-            }
+            if (!(ls == 0 ? PV(ls_).start(p1, p2) : PV(ls_).step(p1, p2))) PV(lsact_) = 0;
           }
         LANES_END
       }
       LANES_BEGIN
         if (PV(act_)) {
-          const float al = PV(alpha_);
+          const float al = PV(ls_).alpha;
           if (!(al > 0.f)) PV(act_) = 0;
           else {
-            PV(impr_) = -0.5f * al * PV(p10_);
+            PV(impr_) = PV(ls_).impr();
             for (int k = 0; k < 6; ++k) PV(x_)[k] += al * PV(sd_)[k];
             PV(iter_) += 1;
             // the next pass would stop on this same test before doing anything with its gradient: stop now and spare the
@@ -2064,8 +1981,8 @@ FE_FN void fe_solve_parts_grouped(FeWarp* w, unsigned skipmask) {
 
 // ---- FAST scope, robot block whose only constraint rows are joint limits (no robot contact): the common case, e.g. the
 // gripper fingers resting on their stops.  Lane d owns dof d in registers; M products are 9 shuffles + 9 FMAs per lane,
-// reductions are xor-butterflies, only the small Cholesky goes through the slice.  Same cost function, stop tests and exact
-// line search as fe_solve_coop.
+// reductions are xor-butterflies, only the small Cholesky goes through the slice.  Same cost function as fe_solve_coop, with
+// the stop test fe_newton_stop and the exact line search FeLineSearch that every Newton solver here uses.
 FE_FN void fe_solve_robot_limits(FeWarp* w) {
   const fe_model* m = w->m;
   const int nr = m->nr, maxit = w->opt.newton_iters, maxls = w->opt.ls_iters;
@@ -2112,9 +2029,7 @@ FE_FN void fe_solve_robot_limits(FeWarp* w) {
     FE_WSUM(a_);
     const float gnorm = sqrtf(FE_UNI(a_));
     if (!(gnorm == gnorm)) { LANES_BEGIN if (lane == 0) w->u()[2] |= 2; LANES_END break; }
-    if (iter > 0) { if (scale * impr < tol || scale * gnorm < tol) break; }
-    else if (scale * gnorm < tol) break;
-    if (iter >= maxit) break;
+    if (fe_newton_stop(iter, maxit, scale, impr, gnorm, tol)) break;
     LANES_BEGIN
       if (lane < nr) { w->Mv()[lane] = PV(u_); w->search()[lane] = -PV(t_); } // H = Mr + diag(D of the active limit rows)
     LANES_END
@@ -2127,10 +2042,9 @@ FE_FN void fe_solve_robot_limits(FeWarp* w) {
     REGS_BEGIN PV(a_) = PV(s_) * PV(r_); PV(b_) = 0.5f * PV(s_) * PV(Ms_); REGS_END
     FE_WSUM(a_); FE_WSUM(b_);
     const float g1 = FE_UNI(a_), g2 = FE_UNI(b_);
-    // exact line search: safeguarded Newton on p'(alpha) = 0
-    float p1 = 0.f, p2 = 0.f, lo = 0.f, hi = -1.f, alpha = 0.f, p1_0 = 0.f, dxold = 0.f;
-    bool fail = false;
-    for (int ls = -1; ls < maxls; ++ls) {
+    FeLineSearch ls; // evaluation -1 is at alpha = 0
+    for (int k = -1; k < maxls; ++k) {
+      const float alpha = ls.alpha;
       REGS_BEGIN
         const float jv = PV(sg_) * PV(s_), xx = PV(sg_) * PV(x_) - PV(ar_) + alpha * jv;
         const bool act = PV(sg_) != 0.f && xx < 0.f;
@@ -2138,26 +2052,12 @@ FE_FN void fe_solve_robot_limits(FeWarp* w) {
         PV(b_) = act ? PV(D_) * jv * jv : 0.f;
       REGS_END
       FE_WSUM(a_); FE_WSUM(b_);
-      p1 = g1 + 2.f * g2 * alpha + FE_UNI(a_);
-      p2 = 2.f * g2 + FE_UNI(b_);
-      if (ls < 0) {
-        if (!(p1 < 0.f) || !(p2 > 0.f)) { fail = true; break; }
-        p1_0 = p1;
-        alpha = -p1 / p2;
-        dxold = alpha;
-        continue;
-      }
-      if (fabsf(p1) <= FE_LS_TOL * fabsf(p1_0)) break;
-      if (p1 < 0.f) lo = alpha; else hi = alpha;
-      float next = alpha - p1 / p2;
-      if (hi > 0.f && (!(next > lo && next < hi) || fabsf(2.f * p1) > fabsf(dxold * p2))) next = 0.5f * (lo + hi); // rtsafe rule
-      if (hi < 0.f && !(next > lo)) next = 2.f * alpha;
-      if (fabsf(next - alpha) <= 1e-6f * fabsf(alpha)) { alpha = next; break; }
-      dxold = fabsf(next - alpha);
-      alpha = next;
+      const float p1 = g1 + 2.f * g2 * alpha + FE_UNI(a_), p2 = 2.f * g2 + FE_UNI(b_);
+      if (!(k < 0 ? ls.start(p1, p2) : ls.step(p1, p2))) break;
     }
-    if (fail || !(alpha > 0.f)) break;
-    impr = -0.5f * alpha * p1_0;
+    const float alpha = ls.alpha;
+    if (!(alpha > 0.f)) break;
+    impr = ls.impr();
     REGS_BEGIN PV(x_) += alpha * PV(s_); PV(r_) += alpha * PV(Ms_); REGS_END
     ++iter;
   }

@@ -18,7 +18,7 @@
 // Exchange between roles goes through small staging arrays of the slice (link twists / wrenches, world-frame contact
 // forces); there is no scan over all contacts and no Hessian in shared memory inside the iteration.  H = M + sum over link
 // pairs of D^T K D is assembled in registers from the constant part (M and the weld terms, packed once per solve) and one
-// 6x6 matrix K per pair of links in contact (the scheme of fe_newton_regs), factored and solved by shuffles.
+// 6x6 matrix K per pair of links in contact (as in fe_newton_regs), factored and solved in registers by FE_REG_CHOL_SOLVE.
 #pragma once
 
 template <int NMAX>
@@ -27,7 +27,7 @@ FE_FN void fe_solve_comp(FeWarp* w, int nA, int ncc, unsigned cplmask, int robot
   const int nr = m->nr, nrl = m->nrlink, nl = m->nlink, np = m->npart, ne = m->neq, nv = m->nv;
   const int maxit = w->opt.newton_iters, maxls = w->opt.ls_iters;
   const float tol = w->opt.tolerance, scale = 1.0f / (m->meaninertia * (float)(nv > 1 ? nv : 1));
-  const float Prx = m->robot_ref[0], Pry = m->robot_ref[1], Prz = m->robot_ref[2];
+  const float Pr[3] = {m->robot_ref[0], m->robot_ref[1], m->robot_ref[2]};
   int* const ccl = (int*)w->Jc(); // [32] component contacts (set by the caller)
   int* const lidx = ccl + 32;     // [64] per-link contact lists: contact | side << 8 (side 1 = the link is the B side)
   int* const lptr = w->first();   // [nlink + 1]
@@ -206,12 +206,8 @@ FE_FN void fe_solve_comp(FeWarp* w, int nA, int ncc, unsigned cplmask, int robot
     if (anyweld)                                                                                                                   \
       for (int e = lane; e < ne; e += 32) {                                                                                        \
         if (!w->eq_active()[e]) continue;                                                                                          \
-        const float *XA = w->lacc2() + 6 * m->eq_link1[e], *XB = w->lacc2() + 6 * m->eq_link2[e];                                 \
-        float t[3], dw[3], rr[6];                                                                                                  \
-        v3cross(t, XA, w->w_r1() + 3 * e);                                                                                         \
-        for (int q = 0; q < 3; ++q) rr[q] = XA[3 + q] + t[q] - XB[3 + q];                                                          \
-        v3sub(dw, XA, XB);                                                                                                         \
-        m3mulv(rr + 3, w->w_G() + 9 * e, dw);                                                                                      \
+        float rr[6];                                                                                                               \
+        fe_weld_rows(w, e, rr);                                                                                                    \
         for (int q = 0; q < 6; ++q) (wdst)[6 * e + q] = rr[q] - ((sub) ? w->w_aref()[6 * e + q] : 0.f);                            \
       }                                                                                                                            \
   LANES_END
@@ -273,7 +269,7 @@ FE_FN void fe_solve_comp(FeWarp* w, int nA, int ncc, unsigned cplmask, int robot
   float impr = 0.f;
   FE_PRIVA(float, row_, NMAX);
   FE_PRIVA(float, kq_, 21); FE_PRIVA(float, d_, 6); FE_PRIVA(float, u_, 6);
-  FE_PRIV(float, s0_); FE_PRIV(float, s1_); FE_PRIV(float, dinv_); FE_PRIV(float, q_); FE_PRIV(float, ks_); FE_PRIV(float, kf_);
+  FE_PRIV(float, ks_); FE_PRIV(float, kf_);
   FE_PRIV(int, bad_);
   for (;;) {
     // cone zone, force and cost of every contact; its share K = G^T W G of the pair's 6x6 matrix; world-frame force staged
@@ -337,20 +333,8 @@ FE_FN void fe_solve_comp(FeWarp* w, int nA, int ncc, unsigned cplmask, int robot
           Wr[0] += sg * t[0]; Wr[1] += sg * t[1]; Wr[2] += sg * t[2]; Wr[3] += sg * fw[0]; Wr[4] += sg * fw[1]; Wr[5] += sg * fw[2];
         }
         if (anyweld && l >= nrl)
-          for (int e = 0; e < ne; ++e) {
-            if (!w->eq_active()[e]) continue;
-            const int A = m->eq_link1[e], B = m->eq_link2[e];
-            if (A != l && B != l) continue;
-            const float* f = w->w_f() + 6 * e;
-            float tq[3], t[3];
-            m3tmulv(tq, w->w_G() + 9 * e, f + 3);
-            if (A == l) {
-              v3cross(t, w->w_r1() + 3 * e, f);
-              Wr[0] += t[0] + tq[0]; Wr[1] += t[1] + tq[1]; Wr[2] += t[2] + tq[2]; Wr[3] += f[0]; Wr[4] += f[1]; Wr[5] += f[2];
-            } else {
-              Wr[0] -= tq[0]; Wr[1] -= tq[1]; Wr[2] -= tq[2]; Wr[3] -= f[0]; Wr[4] -= f[1]; Wr[5] -= f[2];
-            }
-          }
+          for (int e = 0; e < ne; ++e)
+            if (w->eq_active()[e]) fe_weld_wrench(w, e, l, Wr);
         for (int q = 0; q < 6; ++q) w->lacc2()[6 * l + q] = Wr[q];
       }
     LANES_END
@@ -371,14 +355,11 @@ FE_FN void fe_solve_comp(FeWarp* w, int nA, int ncc, unsigned cplmask, int robot
     FE_TICK(w->u(), 27)
     const float cost = FE_UNI(a_), gnorm = sqrtf(FE_UNI(b_));
     if (!(cost == cost)) { LANES_BEGIN if (lane == 0) w->u()[2] |= 2; LANES_END break; }
-    if (iter > 0) { if (scale * impr < tol || scale * gnorm < tol) break; }
-    else if (scale * gnorm < tol) break;
-    if (iter >= maxit) break;
+    if (fe_newton_stop(iter, maxit, scale, impr, gnorm, tol)) break;
 
     // ---- Newton direction: H rows in registers
     REGS_BEGIN
       const int i = lane, zi = PV(z_);
-      PV(bad_) = 0; PV(dinv_) = 1.f;
       const float* Hi = Hm + fe_tri(zi >= 0 ? zi : 0);
 #pragma unroll
       for (int j = 0; j < NMAX; ++j) {
@@ -406,33 +387,11 @@ FE_FN void fe_solve_comp(FeWarp* w, int nA, int ncc, unsigned cplmask, int robot
         FE_SHFL(ks_, PV_ALL(kf_), g);
         const int gkey = (int)FE_UNI(ks_), A = (gkey & 255) - 1, B = (gkey >> 8) - 1;
         const int mA = (A >= 0 && A < nrl) ? m->link_ancmask[A] : 0, mB = (B >= 0 && B < nrl) ? m->link_ancmask[B] : 0;
+        const float p0[3] = {p0x, p0y, p0z};
         REGS_BEGIN // this lane's dof: its unit contribution to the relative twist of the pair (B side minus A side), at p0
-          const int z = PV(z_);
-          float d[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-          if (z >= 0 && z < nr) {
-            const float sg = (float)((mB >> z) & 1) - (float)((mA >> z) & 1);
-            if (sg != 0.f) {
-              const float* S = w->S() + 6 * z;
-              const float r[3] = {p0x - Prx, p0y - Pry, p0z - Prz};
-              float t[3];
-              v3cross(t, S, r);
-              d[0] = sg * S[0]; d[1] = sg * S[1]; d[2] = sg * S[2]; d[3] = sg * (S[3] + t[0]); d[4] = sg * (S[4] + t[1]); d[5] = sg * (S[5] + t[2]);
-            }
-          } else if (z >= nr) {
-            const int part = (z - nr) / 6, jj = (z - nr) % 6, l = nrl + part;
-            const float sg = l == B ? 1.f : (l == A ? -1.f : 0.f);
-            if (sg != 0.f) {
-              if (jj < 3) {
-                const float e[3] = {jj == 0 ? 1.f : 0.f, jj == 1 ? 1.f : 0.f, jj == 2 ? 1.f : 0.f};
-                const float r[3] = {p0x - w->lpos()[3 * l], p0y - w->lpos()[3 * l + 1], p0z - w->lpos()[3 * l + 2]};
-                float t[3];
-                v3cross(t, e, r);
-                d[0] = sg * e[0]; d[1] = sg * e[1]; d[2] = sg * e[2]; d[3] = sg * t[0]; d[4] = sg * t[1]; d[5] = sg * t[2];
-              } else { d[3] = jj == 3 ? sg : 0.f; d[4] = jj == 4 ? sg : 0.f; d[5] = jj == 5 ? sg : 0.f; } // selects keep d in registers
-            }
-          }
+          fe_unit_twist(w, PV(z_), A, B, mA, mB, p0, Pr, PV(d_));
 #pragma unroll
-          for (int q = 0; q < 6; ++q) { PV(d_)[q] = d[q]; PV(u_)[q] = 0.f; }
+          for (int q = 0; q < 6; ++q) PV(u_)[q] = 0.f;
         REGS_END
         // u_i = K d_i, K[a][b] = sum of the members' terms
 #pragma unroll
@@ -459,40 +418,7 @@ FE_FN void fe_solve_comp(FeWarp* w, int nA, int ncc, unsigned cplmask, int robot
       }
     }
     FE_TICK(w->u(), 28)
-    // right-looking Cholesky, pivot column broadcast by shuffle
-#pragma unroll
-    for (int k = 0; k < NMAX; ++k) {
-      FE_SHFLA(s0_, row_, k, k);
-      REGS_BEGIN
-        float pk = PV(s0_);
-        if (!(pk > 1e-30f)) { PV(bad_) = 1; pk = 1e-30f; }
-        const float lkk = sqrtf(pk), inv = 1.0f / lkk;
-        const float lik = lane > k ? PV(row_)[k] * inv : (lane == k ? lkk : 0.f);
-        PV(row_)[k] = lik;
-        PV(q_) = lik;
-        if (lane == k) PV(dinv_) = inv;
-      REGS_END
-#pragma unroll
-      for (int j = k + 1; j < NMAX; ++j) {
-        FE_SHFL(s1_, q_, j);
-        REGS_BEGIN PV(row_)[j] -= PV(q_) * PV(s1_); REGS_END
-      }
-    }
-#pragma unroll
-    for (int k = 0; k < NMAX; ++k) { // y = L^-1 b
-      REGS_BEGIN PV(q_) = PV(b_) * PV(dinv_); REGS_END
-      FE_SHFL(s0_, q_, k);
-      REGS_BEGIN
-        if (lane > k) PV(b_) -= PV(row_)[k] * PV(s0_);
-        else if (lane == k) PV(b_) = PV(s0_);
-      REGS_END
-    }
-#pragma unroll
-    for (int k = NMAX - 1; k >= 0; --k) { // x = L^-T y
-      REGS_BEGIN PV(q_) = (lane > k && lane < NMAX) ? PV(row_)[k] * PV(b_) : 0.f; REGS_END
-      FE_WSUM(q_);
-      REGS_BEGIN if (lane == k) PV(b_) = (PV(b_) - PV(q_)) * PV(dinv_); REGS_END
-    }
+    FE_REG_CHOL_SOLVE(NMAX, row_, b_, bad_)
     LANES_BEGIN
       PV(s_) = PV(z_) >= 0 ? PV(b_) : 0.f;
       if (PV(z_) >= 0) w->search()[PV(z_)] = PV(s_);
@@ -506,28 +432,12 @@ FE_FN void fe_solve_comp(FeWarp* w, int nA, int ncc, unsigned cplmask, int robot
     FE_WSUM(a_); FE_WSUM(b_);
     const float g1 = FE_UNI(a_), g2 = FE_UNI(b_);
     FE_TICK(w->u(), 30)
-    // exact line search: safeguarded Newton on p'(alpha) = 0 (rtsafe rule: bisect unless the step at least halves)
-    float p1 = 0.f, p2 = 0.f, lo = 0.f, hi = -1.f, alpha = 0.f, p1_0 = 0.f, dxold = 0.f;
-    bool fail = false;
-    for (int ls = -1; ls < maxls; ++ls) {
+    FeLineSearch ls; // evaluation -1 is at alpha = 0
+    for (int k = -1; k < maxls; ++k) {
+      const float alpha = ls.alpha;
       REGS_BEGIN
         float q1 = 0.f, q2 = 0.f;
-        if (PV(c_) >= 0) {
-          const float mu = PV(par_)[2], fr = PV(par_)[3], D0 = PV(par_)[0], D1 = PV(par_)[1];
-          const float v0 = PV(jv_)[0], v1 = PV(jv_)[1], v2 = PV(jv_)[2];
-          const float x0 = PV(jar_)[0] + alpha * v0, x1 = PV(jar_)[1] + alpha * v1, x2 = PV(jar_)[2] + alpha * v2;
-          const float N = x0 * mu, U1 = x1 * fr, U2 = x2 * fr, T = sqrtf(U1 * U1 + U2 * U2);
-          if (N >= mu * T || (T <= 0.f && N >= 0.f)) {
-          } else if (mu * N + T <= 0.f || (T <= 0.f && N < 0.f)) {
-            q1 = D0 * x0 * v0 + D1 * (x1 * v1 + x2 * v2);
-            q2 = D0 * v0 * v0 + D1 * (v1 * v1 + v2 * v2);
-          } else {
-            const float Dm = D0 / (mu * mu * (1.f + mu * mu)), NmT = N - mu * T, N1 = v0 * mu, V1 = v1 * fr, V2 = v2 * fr;
-            const float T1 = (U1 * V1 + U2 * V2) / T, T2 = (V1 * V1 + V2 * V2 - T1 * T1) / T, a = N1 - mu * T1;
-            q1 = Dm * NmT * a;
-            q2 = Dm * (a * a - NmT * mu * T2);
-          }
-        }
+        if (PV(c_) >= 0) FE_CONE_LS(PV(jar_), PV(jv_), alpha, PV(par_)[2], PV(par_)[3], PV(par_)[0], PV(par_)[1], q1, =, q2)
         if (anyweld)
           for (int e = lane; e < ne; e += 32) {
             if (!w->eq_active()[e]) continue;
@@ -543,27 +453,13 @@ FE_FN void fe_solve_comp(FeWarp* w, int nA, int ncc, unsigned cplmask, int robot
         PV(a_) = q1; PV(b_) = q2;
       REGS_END
       FE_WSUM(a_); FE_WSUM(b_);
-      p1 = FE_UNI(a_) + g1 + 2.f * alpha * g2;
-      p2 = FE_UNI(b_) + 2.f * g2;
-      if (ls < 0) {
-        if (!(p1 < 0.f) || !(p2 > 0.f)) { fail = true; break; }
-        p1_0 = p1;
-        alpha = -p1 / p2;
-        dxold = alpha;
-        continue;
-      }
-      if (fabsf(p1) <= FE_LS_TOL * fabsf(p1_0)) break;
-      if (p1 < 0.f) lo = alpha; else hi = alpha;
-      float next = alpha - p1 / p2;
-      if (hi > 0.f && (!(next > lo && next < hi) || fabsf(2.f * p1) > fabsf(dxold * p2))) next = 0.5f * (lo + hi);
-      if (hi < 0.f && !(next > lo)) next = 2.f * alpha;
-      if (fabsf(next - alpha) <= 1e-6f * fabsf(alpha)) { alpha = next; break; }
-      dxold = fabsf(next - alpha);
-      alpha = next;
+      const float p1 = FE_UNI(a_) + g1 + 2.f * alpha * g2, p2 = FE_UNI(b_) + 2.f * g2;
+      if (!(k < 0 ? ls.start(p1, p2) : ls.step(p1, p2))) break;
     }
     FE_TICK(w->u(), 31)
-    if (fail || !(alpha > 0.f)) break;
-    impr = -0.5f * alpha * p1_0;
+    const float alpha = ls.alpha;
+    if (!(alpha > 0.f)) break;
+    impr = ls.impr();
     LANES_BEGIN
       PV(x_) += alpha * PV(s_); PV(r_) += alpha * PV(Ms_);
 #pragma unroll

@@ -72,19 +72,6 @@ FE_HD float fe_sum32(const float* scr) {
   return t[0];
 #endif
 }
-FE_HD float fe_min32(const float* scr) {
-#if FE_DEVICE_BUILD
-  float v = scr[threadIdx.x & 31u];
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = fminf(v, __shfl_xor_sync(0xffffffffu, v, o));
-  __syncwarp();
-  return v;
-#else
-  float v = scr[0];
-  for (int i = 1; i < 32; ++i) v = fminf(v, scr[i]);
-  return v;
-#endif
-}
 // bit i set iff flag[i] != 0
 FE_HD unsigned fe_ballot32(const int* flag) {
 #if FE_DEVICE_BUILD
@@ -95,13 +82,6 @@ FE_HD unsigned fe_ballot32(const int* flag) {
   unsigned r = 0;
   for (int i = 0; i < 32; ++i) r |= (flag[i] != 0 ? 1u : 0u) << i;
   return r;
-#endif
-}
-FE_HD int fe_popc(unsigned x) {
-#if FE_DEVICE_BUILD
-  return __popc(x);
-#else
-  return __builtin_popcount(x);
 #endif
 }
 
@@ -115,7 +95,6 @@ FE_HD int fe_popc(unsigned x) {
 #define PV_ALL(name) name /* the private value as a collective operand */
 #define FE_GSUM8(name) do { name += __shfl_xor_sync(0xffffffffu, name, 1); name += __shfl_xor_sync(0xffffffffu, name, 2); name += __shfl_xor_sync(0xffffffffu, name, 4); } while (0)
 #define FE_GSUM8_ARR(name, n) do { _Pragma("unroll") for (int k_ = 0; k_ < (n); ++k_) FE_GSUM8(name[k_]); } while (0)
-#define FE_GSUM8_ARRN(name, n, used) do { _Pragma("unroll") for (int k_ = 0; k_ < (used); ++k_) FE_GSUM8(name[k_]); } while (0)
 #define FE_ANY(name) (__any_sync(0xffffffffu, (name) != 0) != 0)
 // sums over the lane's 4-lane unit, or over its 8-lane pair of units where `wide` is set (per-lane flag, equal within a group)
 #define FE_GSUMV(name, wide) do { name += __shfl_xor_sync(0xffffffffu, name, 1); name += __shfl_xor_sync(0xffffffffu, name, 2); \
@@ -152,7 +131,6 @@ static inline void fe_emu_gsumv(float* a, int stride, const int* wide) {
 }
 #define FE_GSUMV_ARRN(name, n, used, wide) do { for (int k_ = 0; k_ < (used); ++k_) fe_emu_gsumv(&name[0][k_], (n), wide); } while (0)
 #define FE_GSUM8_ARR(name, n) do { for (int k_ = 0; k_ < (n); ++k_) fe_emu_gsum8(&name[0][k_], (n)); } while (0)
-#define FE_GSUM8_ARRN(name, n, used) do { for (int k_ = 0; k_ < (used); ++k_) fe_emu_gsum8(&name[0][k_], (n)); } while (0)
 static inline bool fe_emu_any(const int* a) { for (int i = 0; i < 32; ++i) if (a[i]) return true; return false; }
 #define FE_ANY(name) fe_emu_any(name)
 static inline void fe_emu_wsum(float* a) {
