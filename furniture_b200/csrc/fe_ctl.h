@@ -260,6 +260,6 @@ FE_FN void fe_env_ctl_step_one(FeEnv* e, FeCtlArgs ctl, const float* action, flo
     LANES_END
     fe_substep_lockstep(w);
   }
-  const int fail = (w->u()[2] & 8) ? 1 : 0;
+  const int fail = (w->u()[FE_U_FLAGS] & FE_FLAG_DIVERGED) ? 1 : 0;
   fe_env_finish(e, a, act_dim, connect, fail, fail, reward_out, done_out, info_out);
 }

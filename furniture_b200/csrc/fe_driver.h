@@ -14,9 +14,9 @@ struct FeState {
   float *bias;                                                          // [N][nr]  qfrc_bias of the last forward pass
   float *lpos, *lquat, *lvel;                                           // [N][nlink][3|4|6] of the last forward pass
   int *touch;                                                           // [N][npart]
-  int *flags, *ncon, *niter;                                            // [N]
-  int* order;                                                           // [N] slot -> env: envs that were in the coupled (slow) solver scope last step come first and share blocks
-  int* stats;                                                           // [N][FE_NSTAT] per call: parts-solver iterations, coupled substeps, robot-block solves, coop iterations, cycles/16 in kin, collide, assemble, solve, integrate, all barriers, robot-contact substeps, slowest solve, wait at each of the 5 barriers
+  int *flags, *ncon, *niter;                                            // [N]  flags: FE_FLAG_* bits
+  int* order;                                                           // [N] rank -> env: the envs by the predicted work of their next step, heaviest first (written by fe_order_kernel)
+  int* stats;                                                           // [N][FE_NSTAT] per call: the FE_STAT_* columns
 };
 
 // optional dump of one forward pass (all nullable, [N][dim])
@@ -31,7 +31,7 @@ FE_FN void fe_load(FeWarp* w, const FeState& s, int env) {
   LANES_BEGIN
     LD(qpos, m->nq) LD(qvel, m->nv) LD(warm, m->nv) LD(ctrl, m->nu) LD(qfrc_applied, m->nr) LD(gravcomp, m->npart) LD(eq_data, 7 * m->neq) LD(mpos, 3 * m->nmov)
     LD(contype, m->ngeom) LD(conaff, m->ngeom) LD(eq_active, m->neq) LD(bias, m->nr)
-    w->u()[lane] = 0; // 4 + FE_NSTAT <= 32
+    w->u()[lane] = 0; // FE_U_STAT + FE_NSTAT <= 32
   LANES_END
 #undef LD
 }
@@ -42,8 +42,8 @@ FE_FN void fe_store(FeWarp* w, const FeState& s, int env) {
     ST(qpos, m->nq) ST(qvel, m->nv) ST(warm, m->nv) ST(ctrl, m->nu) ST(qfrc_applied, m->nr) ST(gravcomp, m->npart) ST(eq_data, 7 * m->neq) ST(mpos, 3 * m->nmov)
     ST(contype, m->ngeom) ST(conaff, m->ngeom) ST(eq_active, m->neq)
     ST(bias, m->nr) ST(lpos, 3 * m->nlink) ST(lquat, 4 * m->nlink) ST(lvel, 6 * m->nlink) ST(touch, m->npart)
-    if (lane == 0) { s.flags[env] |= w->u()[2]; s.ncon[env] = w->u()[0]; s.niter[env] = w->u()[3]; }
-    if (lane < FE_NSTAT) s.stats[(size_t)env * FE_NSTAT + lane] = w->u()[4 + lane];
+    if (lane == 0) { s.flags[env] |= w->u()[FE_U_FLAGS]; s.ncon[env] = w->u()[FE_U_NCON]; s.niter[env] = w->u()[FE_U_NITER]; }
+    if (lane < FE_NSTAT) s.stats[(size_t)env * FE_NSTAT + lane] = w->u()[FE_U_STAT + lane];
   LANES_END
 #undef ST
 }

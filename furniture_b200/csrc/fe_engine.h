@@ -12,6 +12,7 @@
 // Solver coordinates z: robot joint accelerations, then for every free part the world-frame spatial acceleration
 // [alpha; vdot_origin] (a fixed orthogonal change of variables of the part's qacc, so the Newton iterates coincide).
 #pragma once
+#include "../../include/furniture_b200.h"
 #include "fe_collide.h"
 #include "fe_model.h"
 #include "fe_warp.h"
@@ -52,9 +53,12 @@ struct FeOpt {
   X(x) X(Ma) X(grad) X(search) X(Mv) X(fc) X(H) X(Jc) X(scr) /* solver */
 #define FE_SLICE_I(X) /* int arrays */ \
   X(contype) X(conaff) X(eq_active) X(cand) X(touch) X(c_geom) X(c_link) X(c_state) X(c_kind) X(plist) X(first) X(iscr) X(colmap) X(skip) \
-  X(u) /* uniform scalars: [0]=ncon [1]=ncand [2]=flags [3]=niter [4..]=per-call statistics */
+  X(u) /* uniform scalars: the FE_U_* words */
 
-#define FE_NSTAT 28 /* per-call statistics kept behind the 4 scalars of u */
+#define FE_NSTAT 28 /* per-call statistics: the FE_STAT_* columns of the `stats` field (include/furniture_b200.h) */
+// words of u: the per-call scalars, then the statistics (column c of `stats` in word FE_U_STAT + c)
+enum { FE_U_NCON = 0, FE_U_NCAND = 1, FE_U_FLAGS = 2, FE_U_NITER = 3, FE_U_STAT = 4 };
+static_assert(FE_STAT_NEWTON_LS < FE_NSTAT && FE_U_STAT + FE_NSTAT <= 32, "u holds every column and is cleared by one lane each");
 struct FeLayout {
 #define X(f) int f;
   FE_SLICE_F(X) FE_SLICE_I(X)
@@ -116,7 +120,7 @@ FE_BOTH int fe_layout_build(FeLayout* L, const fe_model* m, const FeOpt& opt) {
   CARVE(l_sign, nr) CARVE(l_aref, nr) CARVE(l_D, nr) CARVE(l_jar, nr) CARVE(l_jv, nr) CARVE(l_f, nr)
   CARVE(x, nv) CARVE(Ma, nv) CARVE(grad, nv) CARVE(search, nv) CARVE(Mv, nv) CARVE(fc, nv)
   L->Jc = L->lcrb; /* composite inertias (smooth stage) vs row staging of fe_build_H */
-  CARVE(scr, 2 * 32) CARVE(first, nv) CARVE(skip, nv) CARVE(iscr, 32) CARVE(colmap, 32) CARVE(u, 4 + FE_NSTAT)
+  CARVE(scr, 2 * 32) CARVE(first, nv) CARVE(skip, nv) CARVE(iscr, 32) CARVE(colmap, 32) CARVE(u, FE_U_STAT + FE_NSTAT)
   // H (solver) and the collision scratch (geom poses, candidate list) are never live together: overlay them
   const int hwords = fe_tri(nv), cwords = 12 * ng + FE_CAND_WORDS;
   L->H = o; L->gpos = o; L->gmat = o + 3 * ng; L->cand = o + 12 * ng;
@@ -269,7 +273,7 @@ FE_FN void fe_chol_blocks(FeWarp* w, float* H, const int* skip) {
       if (skip[sp]) {
         float A[21];
         for (int i = 0; i < 6; ++i) for (int j = 0; j <= i; ++j) A[i * (i + 1) / 2 + j] = H[fe_tri(sp + i) + sp + j];
-        if (!fe_chol6(A)) w->u()[2] |= 4;
+        if (!fe_chol6(A)) w->u()[FE_U_FLAGS] |= FE_FLAG_NEWTON_PIVOT;
         for (int i = 0; i < 6; ++i) for (int j = 0; j <= i; ++j) H[fe_tri(sp + i) + sp + j] = A[i * (i + 1) / 2 + j];
       }
     }
@@ -355,7 +359,7 @@ FE_FN void fe_robot_solve_regs(FeWarp* w, float hdamp, const float* dadd, const 
   FE_REG_CHOL_SOLVE(NMAX, row_, b_, bad_)
   LANES_BEGIN
     if (lane < nr) x[lane] = PV(b_);
-    if (PV(bad_) && lane == 0) w->u()[2] |= flagbit;
+    if (PV(bad_) && lane == 0) w->u()[FE_U_FLAGS] |= flagbit;
   LANES_END
 }
 FE_FN void fe_robot_solve(FeWarp* w, float hdamp, const float* dadd, const float* b, float* x, int flagbit) {
@@ -617,7 +621,7 @@ FE_FN void fe_kin_smooth(FeWarp* w) {
       }
       float A[21], a[6];
       fe_inert_sym6(A, I, 0.f);
-      if (!fe_chol6(A)) w->u()[2] |= 2;
+      if (!fe_chol6(A)) w->u()[FE_U_FLAGS] |= FE_FLAG_NUMERIC;
       for (int k = 0; k < 6; ++k) { w->fs()[z + k] = W[k]; a[k] = W[k]; }
       fe_chol6_solve(A, a);
       for (int k = 0; k < 6; ++k) w->as()[z + k] = a[k];
@@ -625,7 +629,7 @@ FE_FN void fe_kin_smooth(FeWarp* w) {
   LANES_END
   // robot smooth acceleration: as = Mr^-1 fs
   if (nr > 0) {
-    fe_robot_solve(w, 0.f, nullptr, w->fs(), w->as(), 2);
+    fe_robot_solve(w, 0.f, nullptr, w->fs(), w->as(), FE_FLAG_NUMERIC);
   }
   (void)nv;
 }
@@ -789,7 +793,7 @@ FE_FN void fe_collide(FeWarp* w) {
     ncon += w->iscr()[0];
     LANES_BEGIN LANES_END
   }
-  if (ncon > mc) { ncon = mc; LANES_BEGIN if (lane == 0) w->u()[2] |= 1; LANES_END }
+  if (ncon > mc) { ncon = mc; LANES_BEGIN if (lane == 0) w->u()[FE_U_FLAGS] |= FE_FLAG_CONTACT_FULL; LANES_END }
   // touch flags per part: bit0 left finger, bit1 right finger, bit2 floor, bit3 / bit4 the fingers of a second arm (furniture.py:500-520, :1290-1322)
   LANES_BEGIN
     const int p = lane;
@@ -804,7 +808,7 @@ FE_FN void fe_collide(FeWarp* w) {
       }
       w->touch()[p] |= bits; // sensor pairs have set their bits during the narrow phase
     }
-    if (lane == 0) { w->u()[0] = ncon; w->u()[1] = ncand; }
+    if (lane == 0) { w->u()[FE_U_NCON] = ncon; w->u()[FE_U_NCAND] = ncand; }
   LANES_END
   (void)nrl;
 }
@@ -863,7 +867,7 @@ FE_HD void fe_frame_load(const FeWarp* w, int c, float* F) {
 
 FE_FN void fe_assemble(FeWarp* w) {
   const fe_model* m = w->m;
-  const int ncon = w->u()[0], nr = m->nr, ne = m->neq;
+  const int ncon = w->u()[FE_U_NCON], nr = m->nr, ne = m->neq;
   const float h = m->timestep;
   LANES_BEGIN
     for (int c = lane; c < ncon; c += 32) {
@@ -1086,7 +1090,7 @@ FE_FN void fe_mul_M(FeWarp* w, const float* in, float* out) {
 // rows = J_z in  (contacts -> cout[3*c..], welds -> wout[6*e..], limits -> lout[d]); `sub_aref` subtracts aref
 FE_FN void fe_mul_J(FeWarp* w, const float* in, float* cout, float* wout, float* lout, bool sub_aref) {
   const fe_model* m = w->m;
-  const int nr = m->nr, nrl = m->nrlink, nl = w->fast ? m->nrlink : m->nlink, ncon = w->u()[0], ne = w->fast ? 0 : m->neq;
+  const int nr = m->nr, nrl = m->nrlink, nl = w->fast ? m->nrlink : m->nlink, ncon = w->u()[FE_U_NCON], ne = w->fast ? 0 : m->neq;
   const bool fast = w->fast != 0;
   LANES_BEGIN
     const int l = lane;
@@ -1124,7 +1128,7 @@ FE_FN void fe_mul_J(FeWarp* w, const float* in, float* cout, float* wout, float*
 // constraint forces/states from jar; returns the constraint cost
 FE_FN float fe_update(FeWarp* w) {
   const fe_model* m = w->m;
-  const int ncon = w->u()[0], ne = w->fast ? 0 : m->neq, nr = m->nr;
+  const int ncon = w->u()[FE_U_NCON], ne = w->fast ? 0 : m->neq, nr = m->nr;
   const bool fast = w->fast != 0;
   LANES_BEGIN
     float cost = 0.f;
@@ -1155,7 +1159,7 @@ FE_FN float fe_update(FeWarp* w) {
 // out = J_z^T force
 FE_FN void fe_mul_JT(FeWarp* w, float* out) {
   const fe_model* m = w->m;
-  const int nr = m->nr, nrl = m->nrlink, nl = w->fast ? m->nrlink : m->nlink, ncon = w->u()[0], ne = w->fast ? 0 : m->neq;
+  const int nr = m->nr, nrl = m->nrlink, nl = w->fast ? m->nrlink : m->nlink, ncon = w->u()[FE_U_NCON], ne = w->fast ? 0 : m->neq;
   const bool fast = w->fast != 0;
   LANES_BEGIN
     const int l = lane;
@@ -1197,7 +1201,7 @@ FE_FN void fe_mul_JT(FeWarp* w, float* out) {
 // one 1-D cost evaluation along the search direction: returns p'(alpha), p''(alpha) (uniform)
 FE_FN void fe_line_eval(FeWarp* w, float alpha, float g1, float g2, float* d1, float* d2) {
   const fe_model* m = w->m;
-  const int ncon = w->u()[0], ne = w->fast ? 0 : m->neq, nr = m->nr;
+  const int ncon = w->u()[FE_U_NCON], ne = w->fast ? 0 : m->neq, nr = m->nr;
   const bool fast = w->fast != 0;
   LANES_BEGIN
     float p1 = 0.f, p2 = 0.f;
@@ -1292,7 +1296,7 @@ FE_HDN int fe_cone(float j0, float j1, float j2, float mu, float fr, float D0, f
 // fe_newton_regs (they are added to the register-resident rows there).
 FE_FN void fe_build_H(FeWarp* w, bool regs = false) {
   const fe_model* m = w->m;
-  const int nr = m->nr, nrl = m->nrlink, np = w->fast ? 0 : m->npart, nv = w->nact, ncon = w->u()[0], ne = w->fast ? 0 : m->neq;
+  const int nr = m->nr, nrl = m->nrlink, np = w->fast ? 0 : m->npart, nv = w->nact, ncon = w->u()[FE_U_NCON], ne = w->fast ? 0 : m->neq;
   const bool fast = w->fast != 0;
   // envelope: a part row starts at its own block unless it is coupled to the robot or to a lower part
   LANES_BEGIN
@@ -1490,7 +1494,7 @@ FE_FN void fe_build_H(FeWarp* w, bool regs = false) {
 // NMAX (16 / 24 / 32) bounds the unrolled loops; rows and columns beyond nA are padded with the identity.
 template <int NMAX>
 FE_FN void fe_newton_regs(FeWarp* w, int nA) {
-  const int ncon = w->u()[0];
+  const int ncon = w->u()[FE_U_NCON];
   FE_PRIVA(float, row_, NMAX);
   FE_PRIV(float, b_); FE_PRIV(int, z_); FE_PRIV(int, bad_);
   REGS_BEGIN
@@ -1602,7 +1606,7 @@ FE_FN void fe_newton_regs(FeWarp* w, int nA) {
   FE_REG_CHOL_SOLVE(NMAX, row_, b_, bad_)
   LANES_BEGIN
     if (PV(z_) >= 0) w->search()[PV(z_)] = PV(b_);
-    if (PV(bad_) && lane == 0) w->u()[2] |= 4;
+    if (PV(bad_) && lane == 0) w->u()[FE_U_FLAGS] |= FE_FLAG_NEWTON_PIVOT;
   LANES_END
 }
 
@@ -1610,7 +1614,7 @@ FE_FN void fe_newton_regs(FeWarp* w, int nA) {
 FE_FN void fe_solve_coop(FeWarp* w) {
   FE_TICK_START
   const fe_model* m = w->m;
-  const int nr = m->nr, nrl = m->nrlink, np = w->fast ? 0 : m->npart, nv = w->nact, ncon = w->u()[0], ne = w->fast ? 0 : m->neq;
+  const int nr = m->nr, nrl = m->nrlink, np = w->fast ? 0 : m->npart, nv = w->nact, ncon = w->u()[FE_U_NCON], ne = w->fast ? 0 : m->neq;
   const bool fast = w->fast != 0;
   // any constraint at all?
   LANES_BEGIN
@@ -1627,7 +1631,7 @@ FE_FN void fe_solve_coop(FeWarp* w) {
     LANES_END
     return;
   }
-  LANES_BEGIN if (lane == 0) w->u()[6] += 1; LANES_END
+  LANES_BEGIN if (lane == 0) w->u()[FE_U_STAT + FE_STAT_NEWTON_SOLVES] += 1; LANES_END
   const float scale = 1.0f / (m->meaninertia * (float)(m->nv > 1 ? m->nv : 1));
   // warm start candidate (stored in qacc coordinates) -> z coordinates; pick the cheaper of warm / smooth.  The smooth
   // candidate is costed first: the warm start usually wins, and its products (Ma, jar) are then already in place.
@@ -1688,11 +1692,11 @@ FE_FN void fe_solve_coop(FeWarp* w) {
   if (!fast) for (int p = 0; p < m->npart; ++p) if (w->plist()[9 * p + 8] > 8) regs = false; // needs the grouped static-contact path
   int iter = 0;
   float cost = 0.f, impr = 0.f;
-  FE_TICK(w->u(), 25)
+  FE_TICK(w->u() + FE_U_STAT, FE_STAT_NEWTON_SETUP) // this solver's phases in the FE_STAT_NEWTON_* columns: include/furniture_b200.h
   for (;;) {
     const float ccost = fe_update(w);
     fe_mul_JT(w, w->fc());
-    FE_TICK(w->u(), 26)
+    FE_TICK(w->u() + FE_U_STAT, FE_STAT_NEWTON_START)
     LANES_BEGIN
       float s = 0.f, gsq = 0.f;
       for (int i = lane; i < nv; i += 32) {
@@ -1706,17 +1710,17 @@ FE_FN void fe_solve_coop(FeWarp* w) {
     LANES_END
     const float gauss = fe_sum32(w->scr()), gnorm = sqrtf(fe_sum32(w->scr() + 32));
     cost = gauss + ccost;
-    if (!(cost == cost)) { LANES_BEGIN if (lane == 0) w->u()[2] |= 2; LANES_END break; }
+    if (!(cost == cost)) { LANES_BEGIN if (lane == 0) w->u()[FE_U_FLAGS] |= FE_FLAG_NUMERIC; LANES_END break; }
     // MuJoCo stops on scale*(oldcost - cost) < tol; in fp32 that difference of two large costs is round-off, so the
     // improvement is taken from the line search instead: -alpha p'(0) / 2 (exact for a quadratic, the Newton decrement)
     if (fe_newton_stop(iter, w->opt.newton_iters, scale, impr, gnorm, w->opt.tolerance)) break;
-    FE_TICK(w->u(), 27)
+    FE_TICK(w->u() + FE_U_STAT, FE_STAT_NEWTON_GRAD)
     fe_build_H(w, regs);
-    FE_TICK(w->u(), 28)
+    FE_TICK(w->u() + FE_U_STAT, FE_STAT_NEWTON_HESSIAN)
     if (regs) {
       LANES_BEGIN for (int i = lane; i < nv; i += 32) w->search()[i] = -w->grad()[i]; LANES_END
       if (!fast) { fe_chol_blocks(w, w->H(), w->skip()); fe_solve_blocks(w, w->H(), w->skip(), w->search()); }
-      FE_TICK(w->u(), 29)
+      FE_TICK(w->u() + FE_U_STAT, FE_STAT_NEWTON_CHOL)
       if (nA <= 16) fe_newton_regs<16>(w, nA); else if (nA <= 24) fe_newton_regs<24>(w, nA); else fe_newton_regs<32>(w, nA);
     } else {
       const int* skip = nullptr;
@@ -1727,11 +1731,11 @@ FE_FN void fe_solve_coop(FeWarp* w) {
       }
       LANES_BEGIN for (int i = lane; i < nv; i += 32) w->search()[i] = -w->grad()[i]; LANES_END
       if (skip) fe_solve_blocks(w, w->H(), skip, w->search());
-      if (!fe_chol(w, w->H(), w->first(), nv, skip)) { LANES_BEGIN if (lane == 0) w->u()[2] |= 4; LANES_END }
-      FE_TICK(w->u(), 29)
+      if (!fe_chol(w, w->H(), w->first(), nv, skip)) { LANES_BEGIN if (lane == 0) w->u()[FE_U_FLAGS] |= FE_FLAG_NEWTON_PIVOT; LANES_END }
+      FE_TICK(w->u() + FE_U_STAT, FE_STAT_NEWTON_CHOL)
       fe_chol_solve(w, w->H(), w->first(), nv, w->search(), w->Mv(), skip);
     }
-    FE_TICK(w->u(), 30)
+    FE_TICK(w->u() + FE_U_STAT, FE_STAT_NEWTON_PRODUCTS)
     fe_mul_M(w, w->search(), w->Mv());
     fe_mul_J(w, w->search(), w->c_jv(), w->w_jv(), w->l_jv(), false);
     LANES_BEGIN
@@ -1748,7 +1752,7 @@ FE_FN void fe_solve_coop(FeWarp* w) {
       fe_line_eval(w, ls.alpha, g1, g2, &p1, &p2);
       if (!ls.step(p1, p2)) break;
     }
-    FE_TICK(w->u(), 31)
+    FE_TICK(w->u() + FE_U_STAT, FE_STAT_NEWTON_LS)
     const float alpha = ls.alpha;
     if (!(alpha > 0.f)) break;
     impr = ls.impr();
@@ -1768,8 +1772,8 @@ FE_FN void fe_solve_coop(FeWarp* w) {
   }
   fe_update(w);
   fe_mul_JT(w, w->fc());
-  LANES_BEGIN if (lane == 0) { if (iter > w->u()[3]) w->u()[3] = iter; w->u()[7] += iter; } LANES_END
-  FE_TICK(w->u(), 25)
+  LANES_BEGIN if (lane == 0) { if (iter > w->u()[FE_U_NITER]) w->u()[FE_U_NITER] = iter; w->u()[FE_U_STAT + FE_STAT_NEWTON_ITERS] += iter; } LANES_END
+  FE_TICK(w->u() + FE_U_STAT, FE_STAT_NEWTON_SETUP)
 }
 
 
@@ -1895,11 +1899,11 @@ FE_FN void fe_solve_parts_grouped(FeWarp* w, unsigned skipmask) {
           for (int k = 0; k < 6; ++k) { Mx[k] -= w->fs()[z + k]; g[k] = Mx[k] + PV(acc_)[k]; gsq += g[k] * g[k]; }
           const float gnorm = sqrtf(gsq);
           bool stop = true;
-          if (!(gnorm == gnorm)) { if (PV(lead_)) w->u()[2] |= 2; }
+          if (!(gnorm == gnorm)) { if (PV(lead_)) w->u()[FE_U_FLAGS] |= FE_FLAG_NUMERIC; }
           else stop = fe_newton_stop(PV(iter_), maxit, PV(scale_), PV(impr_), gnorm, tol);
           if (stop) PV(act_) = 0;
           else {
-            if (!fe_chol6(H) && PV(lead_)) w->u()[2] |= 4;
+            if (!fe_chol6(H) && PV(lead_)) w->u()[FE_U_FLAGS] |= FE_FLAG_NEWTON_PIVOT;
             for (int k = 0; k < 6; ++k) PV(sd_)[k] = -g[k];
             fe_chol6_solve(H, PV(sd_));
             float Ms[6], g1 = 0.f, g2 = 0.f;
@@ -2001,7 +2005,7 @@ FE_FN void fe_solve_robot_limits(FeWarp* w) {
     LANES_BEGIN if (lane < nr) { w->x()[lane] = PV(as_); w->fc()[lane] = 0.f; w->l_f()[lane] = 0.f; } LANES_END
     return;
   }
-  LANES_BEGIN if (lane == 0) w->u()[6] += 1; LANES_END
+  LANES_BEGIN if (lane == 0) w->u()[FE_U_STAT + FE_STAT_NEWTON_SOLVES] += 1; LANES_END
   // r = M (warm - as); warm start kept only if it is cheaper than the unconstrained acceleration
   for (int j = 0; j < nr; ++j) {
     FE_SHFL(t_, u_, j);
@@ -2028,12 +2032,12 @@ FE_FN void fe_solve_robot_limits(FeWarp* w) {
     REGS_END
     FE_WSUM(a_);
     const float gnorm = sqrtf(FE_UNI(a_));
-    if (!(gnorm == gnorm)) { LANES_BEGIN if (lane == 0) w->u()[2] |= 2; LANES_END break; }
+    if (!(gnorm == gnorm)) { LANES_BEGIN if (lane == 0) w->u()[FE_U_FLAGS] |= FE_FLAG_NUMERIC; LANES_END break; }
     if (fe_newton_stop(iter, maxit, scale, impr, gnorm, tol)) break;
     LANES_BEGIN
       if (lane < nr) { w->Mv()[lane] = PV(u_); w->search()[lane] = -PV(t_); } // H = Mr + diag(D of the active limit rows)
     LANES_END
-    fe_robot_solve(w, 0.f, w->Mv(), w->search(), w->search(), 4);
+    fe_robot_solve(w, 0.f, w->Mv(), w->search(), w->search(), FE_FLAG_NEWTON_PIVOT);
     REGS_BEGIN PV(s_) = lane < nr ? w->search()[lane] : 0.f; PV(Ms_) = 0.f; REGS_END
     for (int j = 0; j < nr; ++j) {
       FE_SHFL(t_, s_, j);
@@ -2067,7 +2071,7 @@ FE_FN void fe_solve_robot_limits(FeWarp* w) {
       const float f = (PV(sg_) != 0.f && jar < 0.f) ? -PV(D_) * jar : 0.f;
       w->x()[lane] = PV(x_); w->fc()[lane] = PV(sg_) * f; w->l_f()[lane] = f; w->l_jar()[lane] = jar;
     }
-    if (lane == 0) { if (iter > w->u()[3]) w->u()[3] = iter; w->u()[7] += iter; }
+    if (lane == 0) { if (iter > w->u()[FE_U_NITER]) w->u()[FE_U_NITER] = iter; w->u()[FE_U_STAT + FE_STAT_NEWTON_ITERS] += iter; }
   LANES_END
 }
 
@@ -2080,7 +2084,7 @@ FE_FN void fe_solve_robot_limits(FeWarp* w) {
 // dofs or 32 contacts falls back to the cooperative shared-memory solver over all dofs (fe_solve_coop).
 FE_FN void fe_solve(FeWarp* w) {
   const fe_model* m = w->m;
-  const int ncon = w->u()[0], ne = m->neq, np = m->npart, nrl = m->nrlink, nr = m->nr;
+  const int ncon = w->u()[FE_U_NCON], ne = m->neq, np = m->npart, nrl = m->nrlink, nr = m->nr;
   FE_TICK_START
   LANES_BEGIN
     int rcon = 0, cpl = 0;
@@ -2100,14 +2104,14 @@ FE_FN void fe_solve(FeWarp* w) {
       for (int e = 0; e < ne; ++e) if (w->eq_active()[e] && (m->eq_link1[e] == l || m->eq_link2[e] == l)) cpl = 1;
     }
     w->iscr()[lane] = cpl; w->colmap()[lane] = rcon;
-    if (lane == 0) w->u()[3] = 0;
+    if (lane == 0) w->u()[FE_U_NITER] = 0;
   LANES_END
   const unsigned cplmask = fe_ballot32(w->iscr());
   const bool robot_in = fe_ballot32(w->colmap()) != 0u;
   if (cplmask == 0u && !robot_in) { // nothing couples two moving blocks and the robot touches nothing
     fe_solve_parts_grouped(w, 0u);
     LANES_BEGIN
-      if (lane == 0) { int mx = 0; for (int p = 0; p < np; ++p) mx = w->iscr()[p] > mx ? w->iscr()[p] : mx; w->u()[3] = mx; w->u()[4] += mx; }
+      if (lane == 0) { int mx = 0; for (int p = 0; p < np; ++p) mx = w->iscr()[p] > mx ? w->iscr()[p] : mx; w->u()[FE_U_NITER] = mx; w->u()[FE_U_STAT + FE_STAT_PART_ITERS] += mx; }
     LANES_END
     fe_solve_robot_limits(w);
     return;
@@ -2121,7 +2125,7 @@ FE_FN void fe_solve(FeWarp* w) {
       for (int p = 0; p < np; ++p)
         if ((cplmask >> p) & 1u) for (int k = 0; k < 6; ++k) { if (n < 32) w->colmap()[n] = nr + 6 * p + k; ++n; }
       w->iscr()[31] = n;
-      if (cplmask) w->u()[5] += 1; else w->u()[14] += 1;
+      if (cplmask) w->u()[FE_U_STAT + FE_STAT_COUPLED] += 1; else w->u()[FE_U_STAT + FE_STAT_ROBOT_ONLY] += 1;
     }
   LANES_END
   const int nA = w->iscr()[31];
@@ -2144,17 +2148,17 @@ FE_FN void fe_solve(FeWarp* w) {
     LANES_BEGIN LANES_END
   }
   if (nA <= 32 && ncc <= 32) {
-    FE_TICK(w->u(), 21)
+    FE_TICK(w->u() + FE_U_STAT, FE_STAT_SOLVE_PRE)
     fe_solve_parts_grouped(w, cplmask);
     LANES_BEGIN
-      if (lane == 0) { int mx = 0; for (int p = 0; p < np; ++p) if (!((cplmask >> p) & 1u)) mx = w->iscr()[p] > mx ? w->iscr()[p] : mx; w->u()[3] = mx; w->u()[4] += mx; }
+      if (lane == 0) { int mx = 0; for (int p = 0; p < np; ++p) if (!((cplmask >> p) & 1u)) mx = w->iscr()[p] > mx ? w->iscr()[p] : mx; w->u()[FE_U_NITER] = mx; w->u()[FE_U_STAT + FE_STAT_PART_ITERS] += mx; }
     LANES_END
     if (!robot_in) fe_solve_robot_limits(w);
-    FE_TICK(w->u(), 22)
+    FE_TICK(w->u() + FE_U_STAT, FE_STAT_SOLVE_GROUPED)
     if (nA <= 16) fe_solve_comp<16>(w, nA, ncc, cplmask, robot_in ? 1 : 0);
     else if (nA <= 24) fe_solve_comp<24>(w, nA, ncc, cplmask, robot_in ? 1 : 0);
     else fe_solve_comp<32>(w, nA, ncc, cplmask, robot_in ? 1 : 0);
-    FE_TICK(w->u(), 23)
+    FE_TICK(w->u() + FE_U_STAT, FE_STAT_SOLVE_COMP)
     return;
   }
   // fallback: cooperative solver in shared memory (all dofs when something couples, else the robot block)
@@ -2163,7 +2167,7 @@ FE_FN void fe_solve(FeWarp* w) {
   if (!coupled) {
     fe_solve_parts_grouped(w, 0u);
     LANES_BEGIN
-      if (lane == 0) { int mx = 0; for (int p = 0; p < np; ++p) mx = w->iscr()[p] > mx ? w->iscr()[p] : mx; w->u()[3] = mx; w->u()[4] += mx; }
+      if (lane == 0) { int mx = 0; for (int p = 0; p < np; ++p) mx = w->iscr()[p] > mx ? w->iscr()[p] : mx; w->u()[FE_U_NITER] = mx; w->u()[FE_U_STAT + FE_STAT_PART_ITERS] += mx; }
     LANES_END
   }
   fe_solve_coop(w);
@@ -2180,7 +2184,7 @@ FE_FN void fe_integrate(FeWarp* w) {
     LANES_BEGIN
       for (int d = lane; d < nr; d += 32) w->grad()[d] = w->fs()[d] + w->fc()[d];
     LANES_END
-    fe_robot_solve(w, h, nullptr, w->grad(), w->grad(), 2);
+    fe_robot_solve(w, h, nullptr, w->grad(), w->grad(), FE_FLAG_NUMERIC);
   }
   LANES_BEGIN
     // warm start for the next step = solver solution, stored in qacc coordinates
@@ -2199,7 +2203,7 @@ FE_FN void fe_integrate(FeWarp* w) {
       v3cpy(w->warm() + da + 3, t);
       float A[21], a[6];
       fe_inert_sym6(A, w->linert() + 10 * l, h * m->dof_damping[da]);
-      if (!fe_chol6(A)) w->u()[2] |= 2;
+      if (!fe_chol6(A)) w->u()[FE_U_FLAGS] |= FE_FLAG_NUMERIC;
       for (int k = 0; k < 6; ++k) a[k] = w->fs()[z + k] + w->fc()[z + k];
       fe_chol6_solve(A, a);
       m3tmulv(t, R, a);
@@ -2217,14 +2221,14 @@ FE_FN void fe_integrate(FeWarp* w) {
       qnormalize(q);
     }
   LANES_END
-  // divergence guard (mj_checkPos / mj_checkVel): NaN or huge values raise bit 3
+  // divergence guard (mj_checkPos / mj_checkVel): NaN or huge values raise FE_FLAG_DIVERGED
   LANES_BEGIN
     int bad = 0;
     for (int i = lane; i < m->nq; i += 32) { float v = w->qpos()[i]; if (!(v == v) || fabsf(v) > 1e6f) bad = 1; }
     for (int i = lane; i < m->nv; i += 32) { float v = w->qvel()[i]; if (!(v == v) || fabsf(v) > 1e6f) bad = 1; }
     w->iscr()[lane] = bad;
   LANES_END
-  if (fe_ballot32(w->iscr()) != 0u) { LANES_BEGIN if (lane == 0) w->u()[2] |= 8; LANES_END }
+  if (fe_ballot32(w->iscr()) != 0u) { LANES_BEGIN if (lane == 0) w->u()[FE_U_FLAGS] |= FE_FLAG_DIVERGED; LANES_END }
 }
 
 FE_FN void fe_forward(FeWarp* w) {
@@ -2241,15 +2245,14 @@ FE_FN void fe_substep(FeWarp* w) {
 // same time, which is what keeps the instruction cache effective for this large, mostly straight-line code.  Only legal
 // where every live warp of the block executes the same number of steps (the nsub loop of an env step).
 FE_FN void fe_substep_lockstep(FeWarp* w) {
-  // the wait at each barrier is counted in slot 13 (all barriers) and in the barrier's own slot 16-20
   FE_TICK_START
-  FE_BLOCK_SYNC; FE_TICK(w->u(), 13, 16) fe_kin_smooth(w); FE_TICK(w->u(), 8)
-  FE_BLOCK_SYNC; FE_TICK(w->u(), 13, 17) fe_collide(w); FE_TICK(w->u(), 9)
-  FE_BLOCK_SYNC; FE_TICK(w->u(), 13, 18) fe_assemble(w); FE_TICK(w->u(), 10)
-  FE_BLOCK_SYNC; FE_TICK(w->u(), 13, 19) fe_solve(w);
+  FE_BLOCK_SYNC; FE_TICK(w->u() + FE_U_STAT, FE_STAT_WAIT, FE_STAT_WAIT_KIN) fe_kin_smooth(w); FE_TICK(w->u() + FE_U_STAT, FE_STAT_KIN)
+  FE_BLOCK_SYNC; FE_TICK(w->u() + FE_U_STAT, FE_STAT_WAIT, FE_STAT_WAIT_COLLIDE) fe_collide(w); FE_TICK(w->u() + FE_U_STAT, FE_STAT_COLLIDE)
+  FE_BLOCK_SYNC; FE_TICK(w->u() + FE_U_STAT, FE_STAT_WAIT, FE_STAT_WAIT_ASSEMBLE) fe_assemble(w); FE_TICK(w->u() + FE_U_STAT, FE_STAT_ASSEMBLE)
+  FE_BLOCK_SYNC; FE_TICK(w->u() + FE_U_STAT, FE_STAT_WAIT, FE_STAT_WAIT_SOLVE) fe_solve(w);
 #if FE_DEVICE_BUILD
-  { const int d_ = (int)((clock64() - t0_) >> 4); if ((threadIdx.x & 31u) == 0 && d_ > w->u()[15]) w->u()[15] = d_; }
+  { const int d_ = (int)((clock64() - t0_) >> 4); if ((threadIdx.x & 31u) == 0 && d_ > w->u()[FE_U_STAT + FE_STAT_SOLVE_MAX]) w->u()[FE_U_STAT + FE_STAT_SOLVE_MAX] = d_; }
 #endif
-  FE_TICK(w->u(), 11)
-  FE_BLOCK_SYNC; FE_TICK(w->u(), 13, 20) fe_integrate(w); FE_TICK(w->u(), 12)
+  FE_TICK(w->u() + FE_U_STAT, FE_STAT_SOLVE)
+  FE_BLOCK_SYNC; FE_TICK(w->u() + FE_U_STAT, FE_STAT_WAIT, FE_STAT_WAIT_INTEGRATE) fe_integrate(w); FE_TICK(w->u() + FE_U_STAT, FE_STAT_INTEGRATE)
 }

@@ -220,6 +220,20 @@ FE_HD double fe_mt_double(uint32_t* mt, int* pos) {
 FE_HD double fe_mt_uniform(uint32_t* mt, int* pos, double lo, double hi) { return ndadd(lo, ndmul(ndsub(hi, lo), fe_mt_double(mt, pos))); }
 
 // ---------------------------------------------------------------- env context of one warp
+// Scratch of the connect path, the re-pin and the auto-reset: values lane 0 hands to the other lanes and to later parts of the step
+struct FeEnvScratchD {
+  double target_quat[4]; // of the aligned connector pair (fe_try_connect_scan -> fe_connect)
+  double body1_pose[7];  // _connected_body1 after the connection: the re-pin moves its group back to this pose
+  double spare_;
+  double lift;           // lowest site z of the two connected groups (floor clearance)
+};
+struct FeEnvScratchI {
+  int aligned;           // fe_try_connect_scan found an aligned pair
+  int repin;             // part to re-pin at body1_pose after the step (_connected_body1), -1 = none
+  int site1, site2;      // sites of the aligned pair
+  int conn1, conn2;      // their connector indices
+  int done;              // the step ends the episode: auto-reset
+};
 struct FeEnv {
   FeWarp* w;      // header of the env's slice
   const fe_scene* sc;
@@ -229,8 +243,8 @@ struct FeEnv {
   int env;
   // smem-resident env scratch
   int* group;     // [npart] union-find parents (furniture.py:2738-2759)
-  int* ei;        // small int scratch: [0]=connected flag [1]=connected_body1 [2]=site1 [3]=site2 [4]=conn idx1 [5]=conn idx2 [6]=fail
-  double* ed;     // double scratch: [0..3] target quat, [4..10] connected_body1 pose
+  FeEnvScratchI* si;
+  FeEnvScratchD* sd;
 };
 
 FE_HD int fe_find(int* g, int i) { while (g[i] != i) i = g[i]; return i; } // path compression does not change results
@@ -309,19 +323,19 @@ FE_HDN double fe_group_min_z(FeEnv* e, int obj) {
 FE_FN void fe_fwd_step(FeEnv* e) { fe_substep(e->w); }
 
 // _try_connect(part1) for arm agents (part2 = None, _num_connect_steps = 0), furniture.py:926-1042.
-// Runs on lane 0; leaves the aligned pair in ei[2..5] and the target quat in ed[0..3]; ei[0] = 1 if aligned.
+// Runs on lane 0; leaves the aligned pair in si->site1 .. conn2 and the target quat in sd->target_quat; si->aligned = 1 if aligned.
 FE_FN void fe_try_connect_scan(FeEnv* e, int part1) {
   FeWarp* w = e->w;
   const fe_scene* sc = e->sc;
   const fe_config* cfg = e->cfg;
   LANES_BEGIN
     if (lane == 0) {
-      e->ei[0] = 0;
+      e->si->aligned = 0;
       const int g1 = fe_find(e->group, part1);
       const int* connected = e->es.site_connected + (size_t)e->env * w->m->nsite;
       const double thr[4] = {cfg->alignment_pos_dist, cfg->alignment_rot_dist_up, cfg->alignment_rot_dist_forward, cfg->alignment_project_dist};
       bool found = w->m->neq > 0; // some weld joins bodies of the two candidate sets (body2_ids = every part)
-      for (int i = 0; i < sc->nconn && found && !e->ei[0]; ++i) {
+      for (int i = 0; i < sc->nconn && found && !e->si->aligned; ++i) {
         if (fe_find(e->group, sc->conn_part[i]) != g1) continue;
         for (int j = 0; j < sc->nconn; ++j) {
           const int s1 = sc->conn_site[i], s2 = sc->conn_site[j];
@@ -332,8 +346,8 @@ FE_FN void fe_try_connect_scan(FeEnv* e, int part1) {
           fe_site_pose_d(w, s1, p1, m1, nullptr);
           fe_site_pose_d(w, s2, p2, m2, nullptr);
           const bool ok = fe_is_aligned_d(p1, m1, p2, m2, sc->conn_nangles[i], sc->conn_cos[i], sc->conn_sin[i], thr, tq, &tq_set);
-          if (tq_set) for (int k = 0; k < 4; ++k) e->ed[k] = tq[k];
-          if (ok) { e->ei[0] = 1; e->ei[2] = s1; e->ei[3] = s2; e->ei[4] = i; e->ei[5] = j; break; }
+          if (tq_set) for (int k = 0; k < 4; ++k) e->sd->target_quat[k] = tq[k];
+          if (ok) { e->si->aligned = 1; e->si->site1 = s1; e->si->site2 = s2; e->si->conn1 = i; e->si->conn2 = j; break; }
         }
       }
     }
@@ -345,7 +359,7 @@ FE_FN void fe_connect(FeEnv* e) {
   FeWarp* w = e->w;
   const fe_model* m = w->m;
   const fe_scene* sc = e->sc;
-  const int s1 = e->ei[2], s2 = e->ei[3], body1 = sc->conn_part[e->ei[4]], body2 = sc->conn_part[e->ei[5]];
+  const int s1 = e->si->site1, s2 = e->si->site2, body1 = sc->conn_part[e->si->conn1], body2 = sc->conn_part[e->si->conn2];
   LANES_BEGIN
     if (lane == 0) {
       int* connected = e->es.site_connected + (size_t)e->env * m->nsite;
@@ -361,7 +375,7 @@ FE_FN void fe_connect(FeEnv* e) {
         double target[7], base[7], sp[3], sq[4];
         fe_site_pose_d(w, s1, sp, nullptr, sq);
         for (int k = 0; k < 3; ++k) target[k] = sp[k];
-        for (int k = 0; k < 4; ++k) target[3 + k] = e->ed[k];
+        for (int k = 0; k < 4; ++k) target[3 + k] = e->sd->target_quat[k];
         fe_site_pose_d(w, s2, sp, nullptr, sq);
         for (int k = 0; k < 3; ++k) base[k] = sp[k];
         for (int k = 0; k < 4; ++k) base[3 + k] = sq[k];
@@ -385,10 +399,10 @@ FE_FN void fe_connect(FeEnv* e) {
     if (lane == 0) {
       double mn = fe_group_min_z(e, body1), mn2 = fe_group_min_z(e, body2);
       if (mn2 < mn) mn = mn2;
-      e->ed[12] = mn;
+      e->sd->lift = mn;
     }
   LANES_END
-  lift = e->ed[12];
+  lift = e->sd->lift;
   if (lift < 0.0) {
     for (int which = 0; which < 2; ++which) { // _move_rotate_object(body, offset, [0,0,0]) incl. the step inside _is_inside
       LANES_BEGIN
@@ -436,9 +450,9 @@ FE_FN void fe_connect(FeEnv* e) {
         }
       }
       e->es.num_connected[e->env] += 1;
-      e->ei[1] = body1; // _connected_body1 and its pose
+      e->si->repin = body1; // _connected_body1 and its pose
       const int qa = m->link_qadr[m->nrlink + body1];
-      for (int k = 0; k < 7; ++k) e->ed[4 + k] = (double)w->qpos()[qa + k];
+      for (int k = 0; k < 7; ++k) e->sd->body1_pose[k] = (double)w->qpos()[qa + k];
     }
   LANES_END
 }
@@ -506,7 +520,7 @@ FE_FN void fe_env_reset_one(FeEnv* e) {
     for (int s = lane; s < m->nsite; s += 32) e->es.site_connected[(size_t)e->env * m->nsite + s] = 0;
     if (lane == 0) {
       e->es.num_connected[e->env] = 0; e->es.prev_num_connected[e->env] = 0; e->es.episode_len[e->env] = 0; e->es.episode_reward[e->env] = 0.f;
-      w->u()[2] = 0;
+      w->u()[FE_U_FLAGS] = 0;
     }
   LANES_END
   LANES_BEGIN
@@ -600,7 +614,7 @@ FE_FN void fe_env_reset_one(FeEnv* e) {
 }
 
 // the per-step flags: no connection found, no re-pin pending, no auto-reset due, no simulation failure yet (lane 0)
-FE_HD void fe_env_clear_flags(FeEnv* e) { e->ei[0] = 0; e->ei[1] = -1; e->ei[6] = 0; e->w->u()[2] = 0; }
+FE_HD void fe_env_clear_flags(FeEnv* e) { e->si->aligned = 0; e->si->repin = -1; e->si->done = 0; e->w->u()[FE_U_FLAGS] = 0; }
 
 // _setup_action + gravity compensation with the low-level action `a` (indexed by act_src) and the gripper action `grip`
 FE_HD void fe_env_controls(FeEnv* e, const float* a, float grip) {
@@ -645,23 +659,23 @@ FE_HD void fe_env_finish(FeEnv* e, const float* a, int act_dim, float connect, i
         for (int p = 0; p < np; ++p) if ((w->touch()[p] & both) == both) { part = p; break; }
         if (part >= 0) {
           fe_try_connect_scan(e, part);
-          if (e->ei[0]) { fe_connect(e); break; }
+          if (e->si->aligned) { fe_connect(e); break; }
         }
       }
     }
-    const int repin = e->ei[1];
+    const int repin = e->si->repin;
     FE_SYNC; // every lane has read the flag before lane 0 clears it
     if (repin >= 0) { // furniture.py:426-436: re-pin the merged group at the recorded pose, one more step
       LANES_BEGIN
         if (lane == 0) {
-          const int b1 = e->ei[1], qa = m->link_qadr[m->nrlink + b1];
-          double tr[3] = {e->ed[4] - (double)w->qpos()[qa], e->ed[5] - (double)w->qpos()[qa + 1], e->ed[6] - (double)w->qpos()[qa + 2]};
-          fe_move_group(e, b1, tr, e->ed + 7, 0.f);
-          e->ei[1] = -1;
+          const int b1 = e->si->repin, qa = m->link_qadr[m->nrlink + b1];
+          double tr[3] = {e->sd->body1_pose[0] - (double)w->qpos()[qa], e->sd->body1_pose[1] - (double)w->qpos()[qa + 1], e->sd->body1_pose[2] - (double)w->qpos()[qa + 2]};
+          fe_move_group(e, b1, tr, e->sd->body1_pose + 3, 0.f);
+          e->si->repin = -1;
         }
       LANES_END
       fe_fwd_step(e);
-      if (w->u()[2] & 8) { fail = 1; fe_env_reset_one(e); }
+      if (w->u()[FE_U_FLAGS] & FE_FLAG_DIVERGED) { fail = 1; fe_env_reset_one(e); }
     }
   }
   // reward (furniture.py:482-541), termination (:440-445, :451-480)
@@ -710,16 +724,16 @@ FE_HD void fe_env_finish(FeEnv* e, const float* a, int act_dim, float connect, i
       done_out[env] = (uint8_t)done;
       if (e->es.packed) { float* pk = e->es.packed + (size_t)env * (sc->obs_dim + 2) + sc->obs_dim; pk[0] = reward; pk[1] = done ? 1.f : 0.f; }
       int32_t* info = info_out + (size_t)env * FE_INFO_DIM;
-      info[0] = nc; info[1] = success; info[2] = fail; info[3] = len; info[4] = w->u()[0]; info[5] = w->u()[3];
+      info[0] = nc; info[1] = success; info[2] = fail; info[3] = len; info[4] = w->u()[FE_U_NCON]; info[5] = w->u()[FE_U_NITER];
       e->es.done[env] = done;
       // An unstable episode resets twice, as the reference does: once inside _do_simulation's except branch
       // (furniture.py:2889-2897) and once more by the VecEnv worker because the step returned done (subproc_vec_env.py:16-20).
       // The second reset zeroes the episode length that _after_step just incremented and consumes its own random draws,
       // so the env's generator stays draw-for-draw on the reference's stream.
-      e->ei[6] = done;
+      e->si->done = done;
     }
   LANES_END
-  if (e->ei[6]) fe_env_reset_one(e); else fe_write_obs(e);
+  if (e->si->done) fe_env_reset_one(e); else fe_write_obs(e);
 }
 
 // FurnitureEnv.step for one env; writes reward / done / info; auto-resets when done (subproc_vec_env.py:16-20)
@@ -733,7 +747,7 @@ FE_FN void fe_env_step_one(FeEnv* e, const float* action, float* reward_out, uin
   const float connect = a[sc->connect_action_index];
   fe_env_controls(e, a, grip);
   for (int i = 0; i < cfg->nsub; ++i) fe_substep_lockstep(w); // _do_simulation, furniture.py:2877-2879
-  const int fail = (w->u()[2] & 8) ? 1 : 0;             // MujocoException path, :2889-2897
+  const int fail = (w->u()[FE_U_FLAGS] & FE_FLAG_DIVERGED) ? 1 : 0; // MujocoException path, :2889-2897
   fe_env_finish(e, a, sc->act_dim, connect, fail, fail, reward_out, done_out, info_out);
 }
 
@@ -743,11 +757,14 @@ FE_FN void fe_env_bind(FeEnv* e, float* slice, const fe_model* m, const fe_scene
   e->w = fe_warp_bind(slice, m, opt);
   e->sc = sc; e->cfg = cfg; e->st = st; e->es = es; e->env = env;
   float* extra = slice + slice_words_physics;
-  e->ed = (double*)extra;            // 16 doubles (8-byte aligned: slices are multiples of 32 words)
-  e->ei = (int*)(extra + 32);        // 8 ints
+  e->sd = (FeEnvScratchD*)extra;     // 8-byte aligned: slices are multiples of 32 words
+  e->si = (FeEnvScratchI*)(extra + 32);
   e->group = (int*)(extra + 40);     // FE_MAXPART ints
 }
 #define FE_ENV_EXTRA_WORDS 64
+static_assert(sizeof(FeEnvScratchD) <= 4 * 32, "the double scratch ends before the int scratch at word 32");
+static_assert(sizeof(FeEnvScratchI) <= 4 * (40 - 32), "the int scratch ends before group at word 40");
+static_assert(40 + FE_MAXPART <= FE_ENV_EXTRA_WORDS, "group ends within the env's extra words");
 FE_FN void fe_env_load_groups(FeEnv* e) {
   const int np = e->w->m->npart;
   LANES_BEGIN for (int p = lane; p < np; p += 32) e->group[p] = e->es.group[(size_t)e->env * np + p]; LANES_END

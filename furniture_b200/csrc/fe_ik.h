@@ -226,7 +226,7 @@ FE_FN void fe_env_ik_step_one(FeEnv* e, FeIkArgs ik, const float* action, float*
     }
     fe_env_controls(e, st->low, grip);
     for (int i = 0; i < e->cfg->nsub; ++i) fe_substep_lockstep(w);
-    if (w->u()[2] & 8) { // _do_simulation's except branch: reset, then the remaining repeats run on the new episode (furniture.py:2889-2897)
+    if (w->u()[FE_U_FLAGS] & FE_FLAG_DIVERGED) { // _do_simulation's except branch: reset, then the remaining repeats run on the new episode (furniture.py:2889-2897)
       fail = 1;
       FE_SYNC;
       if (r + 1 < c->action_repeat) fe_env_reset_one(e); else reset_now = 1;

@@ -72,7 +72,7 @@ extern "C" __global__ void __launch_bounds__(1024) fe_order_kernel(int N, const 
   // predicted work of the next step: the last step's, but an env that was heavy a few steps ago is still suspect
   for (int e = tid; e < N; e += 1024) {
     const int* st = stats + (size_t)e * FE_NSTAT;
-    const float work = (float)st[4] + (float)st[5] + (float)st[6] + (float)st[7] + (float)st[8]; // cycles / 16
+    const float work = (float)st[FE_STAT_KIN] + (float)st[FE_STAT_COLLIDE] + (float)st[FE_STAT_ASSEMBLE] + (float)st[FE_STAT_SOLVE] + (float)st[FE_STAT_INTEGRATE]; // cycles / 16
     pred[e] = fmaxf(work, FE_ORDER_DECAY * pred[e]);
   }
   __syncthreads();

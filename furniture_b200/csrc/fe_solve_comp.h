@@ -242,7 +242,7 @@ FE_FN void fe_solve_comp(FeWarp* w, int nA, int ncc, unsigned cplmask, int robot
   REGS_END                                                                                                                         \
   FE_WSUM(dst);
 
-  FE_TICK(w->u(), 25)
+  FE_TICK(w->u() + FE_U_STAT, FE_STAT_NEWTON_SETUP)
   // ---- the two starting candidates: the unconstrained (smooth) acceleration and the warm start; the cheaper one is kept
   COMP_MULJ(w->as(), jv_, w->w_jv(), true)  // smooth candidate rows in jv_ / w_jv
   COMP_COST(jv_, w->w_jv(), as_, a_)
@@ -263,7 +263,7 @@ FE_FN void fe_solve_comp(FeWarp* w, int nA, int ncc, unsigned cplmask, int robot
     LANES_END
   }
 
-  FE_TICK(w->u(), 26)
+  FE_TICK(w->u() + FE_U_STAT, FE_STAT_NEWTON_START)
   // ---------------------------------------------------------------- Newton iterations
   int iter = 0;
   float impr = 0.f;
@@ -352,9 +352,9 @@ FE_FN void fe_solve_comp(FeWarp* w, int nA, int ncc, unsigned cplmask, int robot
       PV(b_) = g * g;
     LANES_END
     FE_WSUM(a_); FE_WSUM(b_);
-    FE_TICK(w->u(), 27)
+    FE_TICK(w->u() + FE_U_STAT, FE_STAT_NEWTON_GRAD)
     const float cost = FE_UNI(a_), gnorm = sqrtf(FE_UNI(b_));
-    if (!(cost == cost)) { LANES_BEGIN if (lane == 0) w->u()[2] |= 2; LANES_END break; }
+    if (!(cost == cost)) { LANES_BEGIN if (lane == 0) w->u()[FE_U_FLAGS] |= FE_FLAG_NUMERIC; LANES_END break; }
     if (fe_newton_stop(iter, maxit, scale, impr, gnorm, tol)) break;
 
     // ---- Newton direction: H rows in registers
@@ -417,21 +417,21 @@ FE_FN void fe_solve_comp(FeWarp* w, int nA, int ncc, unsigned cplmask, int robot
         }
       }
     }
-    FE_TICK(w->u(), 28)
+    FE_TICK(w->u() + FE_U_STAT, FE_STAT_NEWTON_HESSIAN)
     FE_REG_CHOL_SOLVE(NMAX, row_, b_, bad_)
     LANES_BEGIN
       PV(s_) = PV(z_) >= 0 ? PV(b_) : 0.f;
       if (PV(z_) >= 0) w->search()[PV(z_)] = PV(s_);
-      if (PV(bad_) && lane == 0) w->u()[2] |= 4;
+      if (PV(bad_) && lane == 0) w->u()[FE_U_FLAGS] |= FE_FLAG_NEWTON_PIVOT;
     LANES_END
-    FE_TICK(w->u(), 29)
+    FE_TICK(w->u() + FE_U_STAT, FE_STAT_NEWTON_CHOL)
     // products with the search direction
     COMP_MULM(w->search(), Ms_)
     COMP_MULJ(w->search(), jv_, w->w_jv(), false)
     REGS_BEGIN PV(a_) = PV(s_) * PV(r_); PV(b_) = 0.5f * PV(s_) * PV(Ms_); REGS_END
     FE_WSUM(a_); FE_WSUM(b_);
     const float g1 = FE_UNI(a_), g2 = FE_UNI(b_);
-    FE_TICK(w->u(), 30)
+    FE_TICK(w->u() + FE_U_STAT, FE_STAT_NEWTON_PRODUCTS)
     FeLineSearch ls; // evaluation -1 is at alpha = 0
     for (int k = -1; k < maxls; ++k) {
       const float alpha = ls.alpha;
@@ -456,7 +456,7 @@ FE_FN void fe_solve_comp(FeWarp* w, int nA, int ncc, unsigned cplmask, int robot
       const float p1 = FE_UNI(a_) + g1 + 2.f * alpha * g2, p2 = FE_UNI(b_) + 2.f * g2;
       if (!(k < 0 ? ls.start(p1, p2) : ls.step(p1, p2))) break;
     }
-    FE_TICK(w->u(), 31)
+    FE_TICK(w->u() + FE_U_STAT, FE_STAT_NEWTON_LS)
     const float alpha = ls.alpha;
     if (!(alpha > 0.f)) break;
     impr = ls.impr();
@@ -482,7 +482,7 @@ FE_FN void fe_solve_comp(FeWarp* w, int nA, int ncc, unsigned cplmask, int robot
 #pragma unroll
       for (int q = 0; q < 3; ++q) w->c_jar()[3 * c + q] = PV(jar_)[q];
     }
-    if (lane == 0) { if (iter > w->u()[3]) w->u()[3] = iter; w->u()[7] += iter; w->u()[6] += 1; }
+    if (lane == 0) { if (iter > w->u()[FE_U_NITER]) w->u()[FE_U_NITER] = iter; w->u()[FE_U_STAT + FE_STAT_NEWTON_ITERS] += iter; w->u()[FE_U_STAT + FE_STAT_NEWTON_SOLVES] += 1; }
   LANES_END
 #undef COMP_MULJ
 #undef COMP_MULM

@@ -22,6 +22,13 @@ DEFAULT_LIB = os.path.join(_HERE, "libfurniture_b200.so")
 MAXCONN = 48
 SCENE_MAGIC = 0x46455344
 INFO_DIM = 6
+# bits of the `flags` field and columns of the `stats` field: FE_FLAG_* / FE_STAT_* of include/furniture_b200.h, which says what each means
+FLAG_CONTACT_FULL, FLAG_NUMERIC, FLAG_NEWTON_PIVOT, FLAG_DIVERGED = 1, 2, 4, 8
+STAT_PART_ITERS, STAT_COUPLED, STAT_NEWTON_SOLVES, STAT_NEWTON_ITERS = 0, 1, 2, 3
+STAT_KIN, STAT_COLLIDE, STAT_ASSEMBLE, STAT_SOLVE, STAT_INTEGRATE, STAT_WAIT, STAT_ROBOT_ONLY, STAT_SOLVE_MAX = 4, 5, 6, 7, 8, 9, 10, 11
+STAT_WAIT_KIN, STAT_WAIT_COLLIDE, STAT_WAIT_ASSEMBLE, STAT_WAIT_SOLVE, STAT_WAIT_INTEGRATE = 12, 13, 14, 15, 16
+STAT_SOLVE_PRE, STAT_SOLVE_GROUPED, STAT_SOLVE_COMP, STAT_RESERVED = 17, 18, 19, 20
+STAT_NEWTON_SETUP, STAT_NEWTON_START, STAT_NEWTON_GRAD, STAT_NEWTON_HESSIAN, STAT_NEWTON_CHOL, STAT_NEWTON_PRODUCTS, STAT_NEWTON_LS = 21, 22, 23, 24, 25, 26, 27
 i32, f32, f64 = C.c_int32, C.c_float, C.c_double
 
 
@@ -74,7 +81,7 @@ def auto_maxcon(em: EngineModel) -> int:
     """Contact capacity per env when the config leaves it open.  The reference runs with nconmax=5000 (base.xml:5), i.e.
     never full; the engine keeps contacts in the env's shared-memory slice, so capacity is sized from the scene: four
     contacts per colliding part geom (a box resting on a face) plus 16 for the robot, at least 44, at most 128.  An env
-    that still overflows raises bit 0 of its `flags` field (never silently dropped)."""
+    that still overflows raises FLAG_CONTACT_FULL in its `flags` field (never silently dropped)."""
     fm = em.fm
     part_geoms = sum(1 for g in range(fm.ngeom) if (fm.geom_tag[g] >> 8) & 0x3FFFFF)
     return int(min(128, max(44, 4 * part_geoms + 16)))

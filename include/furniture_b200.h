@@ -36,7 +36,7 @@ typedef struct fe_handle fe_handle;
 
 typedef struct fe_config {
   int32_t struct_bytes;      /* sizeof(fe_config), checked */
-  int32_t maxcon;            /* contact capacity per env (MuJoCo: nconmax, base.xml:5); an env that overflows raises bit 0 of `flags` */
+  int32_t maxcon;            /* contact capacity per env (MuJoCo: nconmax, base.xml:5); an env that overflows raises FE_FLAG_CONTACT_FULL in `flags` */
   int32_t newton_iters;      /* max Newton iterations per mj_step (MuJoCo default 100) */
   int32_t ls_iters;          /* max line-search evaluations per Newton iteration */
   float tolerance;           /* solver tolerance on scaled improvement / gradient (MuJoCo: 1e-8 in double) */
@@ -93,12 +93,60 @@ int fe_sim_forward(fe_handle* h, void* stream);
 int fe_sim_step(fe_handle* h, int nsub, void* stream);
 /* named per-env arrays, host side; bytes must equal n_envs * dim * sizeof(elem). Names: qpos qvel ctrl qfrc_applied
    qacc_warmstart gravcomp eq_data eq_active geom_contype geom_conaffinity mt_state (624 x uint32) mt_pos (read/write); qfrc_bias link_xpos link_xquat
-   link_xmat link_vel touch ncon niter flags + the debug fields of the last fe_sim_forward (read only) */
+   link_xmat link_vel touch ncon niter + the debug fields of the last fe_sim_forward (read only); flags (int32, the FE_FLAG_* bits below;
+   read/write); stats (int32, one per FE_STAT_* column below; read only); order (int32, one per env: the env ids by the predicted work of their
+   next env step, heaviest first, the order in which the step packs envs into blocks) */
 int fe_get_field(fe_handle* h, const char* name, void* dst_host, size_t bytes);
 int fe_set_field(fe_handle* h, const char* name, const void* src_host, size_t bytes);
 int fe_field_dim(fe_handle* h, const char* name, int* dim, int* elem_bytes);
 int fe_get_state(fe_handle* h, float* qpos_host, float* qvel_host);
 int fe_set_state(fe_handle* h, const float* qpos_host, const float* qvel_host);
+
+/* Bits of `flags`.  A call ORs in the bits an env raised during it (the step kernels clear an env's bits when they set its controls
+   and when they reset it); the field keeps them until the caller writes it. */
+#define FE_FLAG_CONTACT_FULL 1 /* the contact capacity (fe_config.maxcon) was reached: the contacts past it were dropped */
+#define FE_FLAG_NUMERIC 2      /* a NaN cost or gradient in a Newton solve, or a non-positive pivot in a part's 6x6 inertia or in the
+                                  robot's mass or integration matrix */
+#define FE_FLAG_NEWTON_PIVOT 4 /* a non-positive pivot in the Cholesky factor of a Newton solve's Hessian (replaced by a tiny one) */
+#define FE_FLAG_DIVERGED 8     /* qpos or qvel NaN or beyond 1e6 after an mj_step: the episode is unstable (fe_env_step resets it) */
+
+/* Columns of `stats`: counters of the env over the last call, zeroed at its start.  A constraint solve runs once per mj_step and per
+   forward pass.  Cycles are clock64() / 16 of the env's warp; FE_STAT_KIN .. FE_STAT_WAIT_INTEGRATE are written by the env steps
+   and fe_sim_step only. */
+#define FE_STAT_PART_ITERS 0      /* Newton iterations of the per-part solver of free parts, max over the parts, summed over the solves */
+#define FE_STAT_COUPLED 1         /* constraint solves whose coupled component holds a free part */
+#define FE_STAT_NEWTON_SOLVES 2   /* Newton solves of the robot block or of the coupled component that had constraint rows */
+#define FE_STAT_NEWTON_ITERS 3    /* Newton iterations of those solves, summed */
+#define FE_STAT_KIN 4             /* cycles in kinematics and smooth dynamics */
+#define FE_STAT_COLLIDE 5         /* cycles in collision detection */
+#define FE_STAT_ASSEMBLE 6        /* cycles assembling the constraint rows */
+#define FE_STAT_SOLVE 7           /* cycles in the constraint solve */
+#define FE_STAT_INTEGRATE 8       /* cycles in integration */
+#define FE_STAT_WAIT 9            /* cycles waiting at the block barriers ahead of the five phases above, all together */
+#define FE_STAT_ROBOT_ONLY 10     /* constraint solves whose coupled component is the robot block alone (it touches something, no part is coupled) */
+#define FE_STAT_SOLVE_MAX 11      /* cycles of the slowest constraint solve */
+#define FE_STAT_WAIT_KIN 12       /* cycles waiting at the barrier ahead of kinematics */
+#define FE_STAT_WAIT_COLLIDE 13   /* ... ahead of collision detection */
+#define FE_STAT_WAIT_ASSEMBLE 14  /* ... ahead of the constraint rows */
+#define FE_STAT_WAIT_SOLVE 15     /* ... ahead of the constraint solve */
+#define FE_STAT_WAIT_INTEGRATE 16 /* ... ahead of integration */
+/* cycles of a constraint solve whose coupled component fits the register solver (at most 32 dofs and 32 contacts): */
+#define FE_STAT_SOLVE_PRE 17      /* finding the component: which parts are coupled, its dofs and its contacts */
+#define FE_STAT_SOLVE_GROUPED 18  /* the per-part solver of the free parts outside it, and the robot's joint limits when the robot is outside it */
+#define FE_STAT_SOLVE_COMP 19     /* the register solver of the component */
+#define FE_STAT_RESERVED 20       /* never written */
+/* cycles in the phases of the register solver of a component: */
+#define FE_STAT_NEWTON_SETUP 21    /* set-up, once per solve */
+#define FE_STAT_NEWTON_START 22    /* choosing the start: the smooth acceleration or the warm start */
+#define FE_STAT_NEWTON_GRAD 23     /* per iteration: forces, J^T f, cost and gradient */
+#define FE_STAT_NEWTON_HESSIAN 24  /* the Hessian rows */
+#define FE_STAT_NEWTON_CHOL 25     /* Cholesky factor and solves */
+#define FE_STAT_NEWTON_PRODUCTS 26 /* M s and J s along the search direction */
+#define FE_STAT_NEWTON_LS 27       /* line search */
+/* The shared-memory solver, which takes a component beyond 32 dofs or 32 contacts, adds its own phases to the same seven columns:
+   set-up, choosing the start and the final forces (21); forces and J^T f (22); cost, gradient and stop test (23); the Hessian (24);
+   the independent part blocks and, where the direction is not computed in registers, the Cholesky factor (25); the Newton
+   direction (26); M s, J s and line search (27). */
 
 /* ---- environment surface (FurnitureEnv / VecEnv) */
 int fe_env_reset(fe_handle* h, const uint8_t* env_mask_dev /* NULL = all */, float* obs_dev, void* stream);

@@ -18,6 +18,19 @@ def declared_functions():
     return sorted(set(re.findall(r"\b(fe_[a-z_0-9]+)\s*\(", src)))
 
 
+def test_flag_bits_and_stat_columns_match_the_header():
+    """the bits of `flags` and the columns of `stats` are defined in the header (FE_FLAG_* / FE_STAT_*); the Python names in
+    furniture_b200.engine must carry the same values, and the columns must number 0..27 once each"""
+    from furniture_b200 import engine
+
+    src = open(HEADER).read()
+    header = {n: int(v, 0) for n, v in re.findall(r"^#define FE_((?:FLAG|STAT)_[A-Z_0-9]+)\s+(\w+)", src, flags=re.M)}
+    python = {n: getattr(engine, n) for n in dir(engine) if n.startswith(("FLAG_", "STAT_"))}
+    assert header == python
+    assert sorted(v for n, v in header.items() if n.startswith("FLAG_")) == [1, 2, 4, 8]
+    assert sorted(v for n, v in header.items() if n.startswith("STAT_")) == list(range(28))
+
+
 @pytest.fixture(scope="module")
 def lib():
     if not os.path.exists(LIB):

@@ -9,6 +9,7 @@ import numpy as np
 import pytest
 
 from furniture_b200 import mjcf
+from furniture_b200.engine import STAT_COUPLED, STAT_NEWTON_SOLVES
 from oracle.oracle import OracleSim
 from parity_util import have_gpu, make_engine, oracle_link_poses, quat_err, settled_state, to_z
 
@@ -178,7 +179,7 @@ def test_joint_limit_rows_match_oracle(sawyer_model, gpu):
     x = eng.get("dbg_x")
     st = eng.get("stats")
     for e in range(4):
-        assert st[e][2] == 1  # the robot block did need a constraint solve
+        assert st[e][STAT_NEWTON_SOLVES] == 1  # the robot block did need a constraint solve
         assert np.abs(x[e][:9] - ref[e]).max() < 2e-5 * max(1.0, np.abs(ref[e]).max()), (e, np.abs(x[e][:9] - ref[e]).max())
 
 
@@ -206,7 +207,7 @@ def test_grasped_part_coupled_solve_matches_oracle(sawyer_model, gpu):
     sim.forward()
     eng.set("qpos", q2); eng.set("qvel", v); eng.set("qacc_warmstart", np.zeros(m.nv))
     eng.forward()
-    assert eng.get("stats")[0][1] == 1  # the coupled scope was taken
+    assert eng.get("stats")[0][STAT_COUPLED] == 1  # the coupled scope was taken
     assert int(eng.get("ncon")[0][0]) == sim.ncon
     _, _, xm = oracle_link_poses(sim, em)
     zs = to_z(m, em, xm, sim.qacc)

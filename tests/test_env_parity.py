@@ -8,6 +8,7 @@ import numpy as np
 import pytest
 
 from furniture_b200 import mjcf
+from furniture_b200.engine import FLAG_CONTACT_FULL
 from oracle import assembly_oracle as A
 from oracle.ref_env import Cfg, OracleFurnitureEnv
 from parity_util import make_engine
@@ -323,8 +324,8 @@ def test_long_random_rollout_stays_physical():
     assert np.abs(parts[:, :, :2]).max() < 3.0
     assert np.abs(np.linalg.norm(parts[:, :, 3:], axis=2) - 1).max() < 1e-4
     flags = eng.get("flags")[:, 0]
-    assert ((flags & ~1) == 0).all(), np.unique(flags)
-    assert (flags & 1).mean() < 0.01
+    assert ((flags & ~FLAG_CONTACT_FULL) == 0).all(), np.unique(flags)
+    assert (flags & FLAG_CONTACT_FULL).mean() < 0.01
     assert unstable <= n // 100
 
 
@@ -393,7 +394,7 @@ def test_single_step_parity_along_a_drifting_rollout(gpu):
             e.episode_len = int(ln[i, 0])
         a = rng.uniform(-1, 1, (n, eng.act_dim)).astype(np.float32)
         obs, rew, done, info = eng.env_step_host(a)
-        assert (eng.get("flags")[:, 0] & ~1 == 0).all()
+        assert (eng.get("flags")[:, 0] & ~FLAG_CONTACT_FULL == 0).all()
         for i, e in enumerate(envs):
             ob, r, d, inf = e.step(a[i].astype(np.float64))
             assert bool(done[i]) == d

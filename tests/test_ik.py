@@ -8,6 +8,7 @@ import pytest
 
 from furniture_b200 import ik as IK
 from furniture_b200 import mjcf
+from furniture_b200.engine import FLAG_DIVERGED
 from oracle import ik_oracle as O
 
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -289,7 +290,7 @@ def test_unstable_ik_step_resets_mid_step_and_once_more_at_the_end(sawyer):
                 e.rng.uniform(-cfg.agent_xyz_rand, cfg.agent_xyz_rand, e.narm)
         s = e.rng.get_state()
         assert s[2] == pos[i] and np.array_equal(s[1], st[i]), i
-    assert np.isfinite(obs).all() and (eng.get("flags")[:, 0] & 8 == 0).all()
+    assert np.isfinite(obs).all() and (eng.get("flags")[:, 0] & FLAG_DIVERGED == 0).all()
     obs, rew, done, info = eng.env_step_host(a)
     assert info[1][3] == 1 and info[0][3] == 2 and not done.any()
     assert np.isfinite(eng.get("ik_state")[1].view(np.float32)[:44]).all()  # the new episode's targets were re-synchronised from a sane pose

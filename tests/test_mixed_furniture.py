@@ -12,6 +12,7 @@ import numpy as np
 import pytest
 
 from furniture_b200 import mjcf
+from furniture_b200.engine import FLAG_CONTACT_FULL
 from oracle.ref_env import OracleFurnitureEnv
 from parity_util import make_engine
 from test_env_parity import _sync_oracle_from_engine
@@ -39,7 +40,7 @@ def _run(name, gpu, n=2, steps=2):
     q = eng.get("qpos")
     assert np.isfinite(q).all()
     if name in UNLISTED:
-        assert ((flags & ~1) == 0).all(), flags  # at most the capacity bit
+        assert ((flags & ~FLAG_CONTACT_FULL) == 0).all(), flags  # at most the capacity bit
         if name in OVERFLOW or (flags != 0).any():  # how deep the panels start inside the floor depends on the draw
             eng.close()
             return

@@ -13,6 +13,7 @@ import numpy as np
 import pytest
 
 from furniture_b200 import mjcf
+from furniture_b200.engine import FLAG_DIVERGED
 from oracle.ref_env import Cfg, OracleFurnitureEnv
 from parity_util import make_engine
 
@@ -136,7 +137,7 @@ def test_unstable_episode_resets_twice_like_the_reference_worker():
                 e.rng.uniform(-cfg.agent_xyz_rand, cfg.agent_xyz_rand, e.narm)
         s = e.rng.get_state()
         assert s[2] == pos[i] and np.array_equal(s[1], st[i]), i
-    assert np.isfinite(obs).all() and (eng.get("flags")[:, 0] & 8 == 0).all()
+    assert np.isfinite(obs).all() and (eng.get("flags")[:, 0] & FLAG_DIVERGED == 0).all()
     obs, rew, done, info = eng.env_step_host(a)
     assert info[1][3] == 1 and info[0][3] == 2 and not done.any()
 

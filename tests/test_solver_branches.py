@@ -23,6 +23,7 @@ import numpy as np
 import pytest
 
 from furniture_b200 import mjcf
+from furniture_b200.engine import FLAG_CONTACT_FULL
 from furniture_b200.engine_model import EngineModel
 from oracle.assembly_oracle import rel_pose
 from oracle.oracle import OracleSim
@@ -315,7 +316,7 @@ def broad_phase_candidates(m, sim):
 
 @pytest.mark.parametrize("gpu", BACKENDS)
 def test_contact_capacity_edges(gpu):
-    """maxcon equal to the oracle's contact count: no flag and full parity; one less: bit 0 of flags, ncon == maxcon, and the
+    """maxcon equal to the oracle's contact count: no flag and full parity; one less: FLAG_CONTACT_FULL, ncon == maxcon, and the
     contacts kept are the oracle's first maxcon in order"""
     m, em, states = pile_states(*SOURCES["lack"])
     s = next(s for s in states if s["branch"] == "comp24" and not s["mpr"])
@@ -327,7 +328,7 @@ def test_contact_capacity_edges(gpu):
     sim = OracleSim(m)
     sim.qpos[:] = s["qpos"]; sim.qvel[:] = s["qvel"]; sim.forward()
     oc = sim.contacts()
-    assert eng.get("flags")[0][0] & 1 and eng.get("ncon")[0][0] == k - 1
+    assert eng.get("flags")[0][0] & FLAG_CONTACT_FULL and eng.get("ncon")[0][0] == k - 1
     kept = [tuple(sorted((int(em.geom_src[g & 255]), int(em.geom_src[g >> 8])))) for g in eng.get("con_geom")[0][: k - 1]]
     assert kept == [tuple(sorted((c.geom1, c.geom2))) for c in oc[: k - 1]]
 

@@ -4,6 +4,7 @@ mixed batch with these numbers instead of the nv^3 guess."""
 import json, os, sys
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
 import torch
+from furniture_b200.engine import FLAG_CONTACT_FULL
 from furniture_b200.env import BatchedFurnitureEnv
 
 ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
@@ -26,7 +27,7 @@ for name in names:
     e1.record(); torch.cuda.synchronize()
     ms = e0.elapsed_time(e1) / 4
     out[name] = {"us_per_env_step": ms * 1e3 / N, "ms_per_step_at_%d" % N: ms, "nv": int(env.model.nv), "smem_bytes_per_env": int(env.engine.L.fe_smem_bytes_per_env(env.engine.h)),
-                 "overflow_envs": int((env.engine.get("flags")[:, 0] & 1).sum())}
+                 "overflow_envs": int((env.engine.get("flags")[:, 0] & FLAG_CONTACT_FULL).sum())}
     print(name, out[name], flush=True)
     env.close()
 json.dump(out, open(os.path.join(ROOT, "gpurun_out", "model_cost.json"), "w"), indent=1)

@@ -3,7 +3,7 @@ import sys, os
 sys.path.insert(0, os.path.join(os.path.dirname(__file__), ".."))
 import numpy as np, torch
 from furniture_b200 import mjcf
-from furniture_b200.engine import Engine, default_config
+from furniture_b200.engine import FLAG_CONTACT_FULL, Engine, default_config
 N = int(sys.argv[1]) if len(sys.argv) > 1 else 4096
 steps = int(sys.argv[2]) if len(sys.argv) > 2 else 30
 m = mjcf.load_scene("Sawyer", "table_lack_0825")
@@ -21,7 +21,7 @@ for k in range(steps):
     hist += np.bincount(np.minimum(nc, 199), minlength=200)
 e1.record(); torch.cuda.synchronize()
 fl = eng.get("flags")[:, 0]
-print("maxcon", eng.cfg.maxcon, "after", steps, "steps: envs with overflow bit", int((fl & 1).sum()), "other bits", int((fl & ~1 != 0).sum()), "of", N)
+print("maxcon", eng.cfg.maxcon, "after", steps, "steps: envs with overflow bit", int((fl & FLAG_CONTACT_FULL).sum()), "other bits", int((fl & ~FLAG_CONTACT_FULL != 0).sum()), "of", N)
 print("ncon at step end: p50 %d p90 %d p99 %d max %d; share of (env,step) with ncon >= 36: %.3f%%, >= 40: %.3f%%" % (
     np.searchsorted(np.cumsum(hist), 0.5 * hist.sum()), np.searchsorted(np.cumsum(hist), 0.9 * hist.sum()), np.searchsorted(np.cumsum(hist), 0.99 * hist.sum()),
     np.nonzero(hist)[0].max(), 100 * hist[36:].sum() / hist.sum(), 100 * hist[40:].sum() / hist.sum()))

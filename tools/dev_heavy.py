@@ -5,6 +5,7 @@ sys.path.insert(0, os.path.join(os.path.dirname(__file__), ".."))
 sys.path.insert(0, os.path.join(os.path.dirname(__file__), "..", "tests"))
 import numpy as np, torch
 from furniture_b200 import mjcf
+from furniture_b200 import engine as E
 from furniture_b200.engine import Engine, default_config
 from oracle.ref_env import OracleFurnitureEnv
 from test_env_parity import _grasp_and_align_state
@@ -30,10 +31,10 @@ for N in [int(a) for a in sys.argv[1:]] or [1, 7, 132 * 7, 4096]:
         eng.env_step_dev(a.data_ptr(), obs.data_ptr(), rew.data_ptr(), done.data_ptr(), info.data_ptr())
     e1.record(); torch.cuda.synchronize()
     st = eng.get("stats").astype(np.float64)
-    nsol, its = st[:, 2].sum(), st[:, 3].sum()
-    cyc = st[:, 4:10] * 16
-    pre = st[:, 17:20] * 16
-    cc = st[:, 21:28] * 16
+    nsol, its = st[:, E.STAT_NEWTON_SOLVES].sum(), st[:, E.STAT_NEWTON_ITERS].sum()
+    cyc = st[:, [E.STAT_KIN, E.STAT_COLLIDE, E.STAT_ASSEMBLE, E.STAT_SOLVE, E.STAT_INTEGRATE, E.STAT_WAIT]] * 16
+    pre = st[:, [E.STAT_SOLVE_PRE, E.STAT_SOLVE_GROUPED, E.STAT_SOLVE_COMP]] * 16
+    cc = st[:, [E.STAT_NEWTON_SETUP, E.STAT_NEWTON_START, E.STAT_NEWTON_GRAD, E.STAT_NEWTON_HESSIAN, E.STAT_NEWTON_CHOL, E.STAT_NEWTON_PRODUCTS, E.STAT_NEWTON_LS]] * 16
     print("N=%d: %.2f ms per env-step batch; solves/env %.0f iterations/solve %.2f ncon %.0f | phases per mj_step: kin %.0f collide %.0f assemble %.0f solve %.0f integrate %.0f wait %.0f" % ((N, e0.elapsed_time(e1) / 3, nsol / N, its / max(nsol, 1), info[:, 4].float().mean().item()) + tuple(cyc.mean(0) / 50)))
     print("   per solve: preamble %.0f grouped+limits %.0f component %.0f (setup %.0f candidates %.0f) | per iteration: forces+JTf+grad %.0f H rows+pairs %.0f cholesky+solves %.0f Ms,Js %.0f line search %.0f" % (tuple(pre.sum(0) / max(nsol, 1)) + tuple(cc[:, :2].sum(0) / max(nsol, 1)) + tuple(cc[:, 2:].sum(0) / max(its, 1))))
     eng.close()
