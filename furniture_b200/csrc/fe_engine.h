@@ -78,12 +78,10 @@ __constant__ FeLayout fe_c_lay;
 #define FE_LAY fe_h_lay
 #endif
 
-#define FE_WARP_HDR_WORDS 10 /* sizeof(FeWarp) is 8 words; the 2 spare words keep every array at the offset the kernels were tuned with */
+#define FE_WARP_HDR_WORDS 10 /* sizeof(FeWarp) is 6 words; the 4 spare words keep every array at the offset the kernels were tuned with */
 struct FeWarp { // header at word 0 of the slice
   const fe_model* m;
   FeOpt opt;
-  // solver scope of the cooperative routines: all dofs (FULL) or the robot block only (FAST, parts solved per lane group)
-  int nact, fast;
   // Device: the slice address is rebuilt from the dynamic shared-memory symbol plus the warp's byte offset, so that the compiler
   // sees a shared-memory pointer and emits LDS / STS with 32-bit addresses (through the generic `this` every slice access was
   // a generic LD.E / ST.E with a 64-bit address pair).
@@ -133,7 +131,7 @@ FE_BOTH int fe_layout_build(FeLayout* L, const fe_model* m, const FeOpt& opt) {
 FE_FN FeWarp* fe_warp_bind(float* slice, const fe_model* m, const FeOpt& opt) {
   FeWarp* w = (FeWarp*)slice;
   LANES_BEGIN
-    if (lane == 0) { w->m = m; w->opt = opt; w->nact = m->nv; w->fast = 0; }
+    if (lane == 0) { w->m = m; w->opt = opt; }
   LANES_END
   return w;
 }
@@ -1077,7 +1075,7 @@ FE_HD void fe_weld_wrench(const FeWarp* w, int e, int l, float* Wr) {
 // out = M_z in
 FE_FN void fe_mul_M(FeWarp* w, const float* in, float* out) {
   const fe_model* m = w->m;
-  const int nr = m->nr, np = w->fast ? 0 : m->npart, nrl = m->nrlink;
+  const int nr = m->nr, np = m->npart, nrl = m->nrlink;
   LANES_BEGIN
     for (int d = lane; d < nr; d += 32) {
       float s = 0.f;
@@ -1090,8 +1088,7 @@ FE_FN void fe_mul_M(FeWarp* w, const float* in, float* out) {
 // rows = J_z in  (contacts -> cout[3*c..], welds -> wout[6*e..], limits -> lout[d]); `sub_aref` subtracts aref
 FE_FN void fe_mul_J(FeWarp* w, const float* in, float* cout, float* wout, float* lout, bool sub_aref) {
   const fe_model* m = w->m;
-  const int nr = m->nr, nrl = m->nrlink, nl = w->fast ? m->nrlink : m->nlink, ncon = w->u()[FE_U_NCON], ne = w->fast ? 0 : m->neq;
-  const bool fast = w->fast != 0;
+  const int nr = m->nr, nrl = m->nrlink, nl = m->nlink, ncon = w->u()[FE_U_NCON], ne = m->neq;
   LANES_BEGIN
     const int l = lane;
     if (l < nl) {
@@ -1106,7 +1103,6 @@ FE_FN void fe_mul_J(FeWarp* w, const float* in, float* cout, float* wout, float*
   LANES_END
   LANES_BEGIN
     for (int c = lane; c < ncon; c += 32) {
-      if (fast && w->c_kind()[c] == 0) continue;
       const int A = (w->c_link()[c] & 255) - 1, B = (w->c_link()[c] >> 8) - 1;
       float aA[3], aB[3], da[3];
       fe_point_vel(w, w->lacc2(), A, w->c_pos() + 3 * c, aA);
@@ -1128,12 +1124,10 @@ FE_FN void fe_mul_J(FeWarp* w, const float* in, float* cout, float* wout, float*
 // constraint forces/states from jar; returns the constraint cost
 FE_FN float fe_update(FeWarp* w) {
   const fe_model* m = w->m;
-  const int ncon = w->u()[FE_U_NCON], ne = w->fast ? 0 : m->neq, nr = m->nr;
-  const bool fast = w->fast != 0;
+  const int ncon = w->u()[FE_U_NCON], ne = m->neq, nr = m->nr;
   LANES_BEGIN
     float cost = 0.f;
     for (int c = lane; c < ncon; c += 32) {
-      if (fast && w->c_kind()[c] == 0) continue;
       float f[3];
       const int st = fe_cone_t<false>(w->c_jar()[3 * c], w->c_jar()[3 * c + 1], w->c_jar()[3 * c + 2], w->c_mu()[c], w->c_fric()[c], w->c_D()[2 * c], w->c_D()[2 * c + 1], f, &cost, nullptr);
       w->c_f()[3 * c] = f[0]; w->c_f()[3 * c + 1] = f[1]; w->c_f()[3 * c + 2] = f[2];
@@ -1159,15 +1153,13 @@ FE_FN float fe_update(FeWarp* w) {
 // out = J_z^T force
 FE_FN void fe_mul_JT(FeWarp* w, float* out) {
   const fe_model* m = w->m;
-  const int nr = m->nr, nrl = m->nrlink, nl = w->fast ? m->nrlink : m->nlink, ncon = w->u()[FE_U_NCON], ne = w->fast ? 0 : m->neq;
-  const bool fast = w->fast != 0;
+  const int nr = m->nr, nrl = m->nrlink, nl = m->nlink, ncon = w->u()[FE_U_NCON], ne = m->neq;
   LANES_BEGIN
     const int l = lane;
     if (l < nl) {
       float P[3], Wr[6] = {0, 0, 0, 0, 0, 0};
       fe_link_ref(w, l, P);
       for (int c = 0; c < ncon; ++c) {
-        if (fast && w->c_kind()[c] == 0) continue;
         if (w->c_state()[c] == 0) continue;
         const int A = (w->c_link()[c] & 255) - 1, B = (w->c_link()[c] >> 8) - 1;
         if (A != l && B != l) continue;
@@ -1201,12 +1193,10 @@ FE_FN void fe_mul_JT(FeWarp* w, float* out) {
 // one 1-D cost evaluation along the search direction: returns p'(alpha), p''(alpha) (uniform)
 FE_FN void fe_line_eval(FeWarp* w, float alpha, float g1, float g2, float* d1, float* d2) {
   const fe_model* m = w->m;
-  const int ncon = w->u()[FE_U_NCON], ne = w->fast ? 0 : m->neq, nr = m->nr;
-  const bool fast = w->fast != 0;
+  const int ncon = w->u()[FE_U_NCON], ne = m->neq, nr = m->nr;
   LANES_BEGIN
     float p1 = 0.f, p2 = 0.f;
     for (int c = lane; c < ncon; c += 32) {
-      if (fast && w->c_kind()[c] == 0) continue;
       FE_CONE_LS(w->c_jar() + 3 * c, w->c_jv() + 3 * c, alpha, w->c_mu()[c], w->c_fric()[c], w->c_D()[2 * c], w->c_D()[2 * c + 1], p1, +=, p2)
     }
     for (int e = lane; e < ne; e += 32) {
@@ -1296,8 +1286,7 @@ FE_HDN int fe_cone(float j0, float j1, float j2, float mu, float fr, float D0, f
 // fe_newton_regs (they are added to the register-resident rows there).
 FE_FN void fe_build_H(FeWarp* w, bool regs = false) {
   const fe_model* m = w->m;
-  const int nr = m->nr, nrl = m->nrlink, np = w->fast ? 0 : m->npart, nv = w->nact, ncon = w->u()[FE_U_NCON], ne = w->fast ? 0 : m->neq;
-  const bool fast = w->fast != 0;
+  const int nr = m->nr, nrl = m->nrlink, np = m->npart, nv = m->nv, ncon = w->u()[FE_U_NCON], ne = m->neq;
   // envelope: a part row starts at its own block unless it is coupled to the robot or to a lower part
   LANES_BEGIN
     for (int d = lane; d < nr; d += 32) w->first()[d] = 0;
@@ -1339,17 +1328,17 @@ FE_FN void fe_build_H(FeWarp* w, bool regs = false) {
       }
     }
   LANES_END
-  // FULL scope: contacts of a free part against the static world only touch that part's 6x6 diagonal block; they are
-  // accumulated 8 lanes per part (lane = contact) with group reductions, like the FAST solver does
-  bool grouped = !fast;
-  for (int p = 0; p < m->npart; ++p) if (w->plist()[9 * p + 8] > 8) grouped = false;
+  // contacts of a free part against the static world only touch that part's 6x6 diagonal block; unless a part has more
+  // than 8 of them, they are accumulated 8 lanes per part (lane = contact) with group reductions, like fe_solve_parts_grouped
+  bool grouped = true;
+  for (int p = 0; p < np; ++p) if (w->plist()[9 * p + 8] > 8) grouped = false;
   if (grouped) {
-    for (int pass = 0; pass * 4 < m->npart; ++pass) {
+    for (int pass = 0; pass * 4 < np; ++pass) {
       FE_PRIVA(float, hacc_, 21);
       LANES_BEGIN
         for (int k = 0; k < 21; ++k) PV(hacc_)[k] = 0.f;
         const int part = pass * 4 + (lane >> 3), slot = lane & 7;
-        if (part < m->npart && slot < w->plist()[9 * part + 8]) {
+        if (part < np && slot < w->plist()[9 * part + 8]) {
           const int c = w->plist()[9 * part + slot];
           if (w->c_state()[c] != 0) {
             const int l = nrl + part, B_ = (w->c_link()[c] >> 8) - 1;
@@ -1369,7 +1358,7 @@ FE_FN void fe_build_H(FeWarp* w, bool regs = false) {
       FE_GSUM8_ARR(hacc_, 21);
       LANES_BEGIN
         const int part = pass * 4 + (lane >> 3);
-        if (part < m->npart && (lane & 7) == 0 && w->plist()[9 * part + 8] > 0) {
+        if (part < np && (lane & 7) == 0 && w->plist()[9 * part + 8] > 0) {
           const int z = nr + 6 * part;
           for (int i = 0; i < 6; ++i) for (int j = 0; j <= i; ++j) w->H()[fe_tri(z + i) + z + j] += PV(hacc_)[i * (i + 1) / 2 + j];
         }
@@ -1379,7 +1368,7 @@ FE_FN void fe_build_H(FeWarp* w, bool regs = false) {
   // remaining contacts, one at a time: dof-space rows staged in Jc (3 x ncols), then the ncols x ncols outer product
   for (int c = 0; c < ncon && !regs; ++c) {
     const int st = w->c_state()[c];
-    if (st == 0 || ((fast || grouped) && w->c_kind()[c] == 0)) continue;
+    if (st == 0 || (grouped && w->c_kind()[c] == 0)) continue;
     const int A = (w->c_link()[c] & 255) - 1, B = (w->c_link()[c] >> 8) - 1;
     const bool robot = (A >= 0 && A < nrl) || (B >= 0 && B < nrl);
     const int partA = A >= nrl ? A - nrl : -1, partB = B >= nrl ? B - nrl : -1;
@@ -1610,16 +1599,16 @@ FE_FN void fe_newton_regs(FeWarp* w, int nA) {
   LANES_END
 }
 
-// cooperative Newton solve over the active scope (w->nact dofs; in FAST scope the free parts are excluded)
-FE_FN void fe_solve_coop(FeWarp* w) {
+// cooperative Newton solve over all dofs.  cplmask: the parts that a constraint couples to another moving block (bit p for
+// part p, as fe_solve decides it); they join the robot dofs in the register-resident Newton direction, the other parts are
+// independent 6x6 blocks.
+FE_FN void fe_solve_coop(FeWarp* w, unsigned cplmask) {
   FE_TICK_START
   const fe_model* m = w->m;
-  const int nr = m->nr, nrl = m->nrlink, np = w->fast ? 0 : m->npart, nv = w->nact, ncon = w->u()[FE_U_NCON], ne = w->fast ? 0 : m->neq;
-  const bool fast = w->fast != 0;
+  const int nr = m->nr, nrl = m->nrlink, np = m->npart, nv = m->nv, ncon = w->u()[FE_U_NCON], ne = m->neq;
   // any constraint at all?
   LANES_BEGIN
-    int any = 0;
-    for (int c = lane; c < ncon; c += 32) any |= !(fast && w->c_kind()[c] == 0);
+    int any = lane < ncon;
     for (int e = lane; e < ne; e += 32) any |= w->eq_active()[e] != 0;
     for (int d = lane; d < nr; d += 32) any |= w->l_sign()[d] != 0.f;
     w->iscr()[lane] = any;
@@ -1663,25 +1652,14 @@ FE_FN void fe_solve_coop(FeWarp* w) {
     fe_mul_M(w, w->x(), w->Ma());
     fe_mul_J(w, w->x(), w->c_jar(), w->w_jar(), w->l_jar(), true);
   }
-  // active set of the register-resident Newton direction: the robot dofs plus every part that a constraint couples to
-  // another moving block (decided by constraint kind, not by contact state, so it is fixed for the whole solve); the
-  // remaining parts are independent 6x6 blocks (skip[] = 1)
-  LANES_BEGIN
-    if (lane < np) {
-      const int l = nrl + lane;
-      int cpl = w->plist()[9 * lane + 8] > 8;
-      for (int c = 0; c < ncon && !cpl; ++c)
-        if (w->c_kind()[c] >= 2) { const int A = (w->c_link()[c] & 255) - 1, B = (w->c_link()[c] >> 8) - 1; cpl = A == l || B == l; }
-      for (int e = 0; e < ne && !cpl; ++e) if (w->eq_active()[e]) cpl = m->eq_link1[e] == l || m->eq_link2[e] == l;
-      w->iscr()[lane] = cpl;
-    }
-  LANES_END
+  // active set of the register-resident Newton direction: the robot dofs, then the coupled parts (fixed for the whole
+  // solve); the remaining parts are independent 6x6 blocks (skip[] = 1)
   LANES_BEGIN
     if (lane == 0) {
       int n = 0;
       for (int d = 0; d < nr; ++d) { w->skip()[d] = 0; if (n < 32) w->colmap()[n] = d; ++n; }
       for (int p = 0; p < np; ++p) {
-        const int cpl = w->iscr()[p];
+        const int cpl = (cplmask >> p) & 1u;
         for (int k = 0; k < 6; ++k) { w->skip()[nr + 6 * p + k] = !cpl; if (cpl) { if (n < 32) w->colmap()[n] = nr + 6 * p + k; ++n; } }
       }
       w->iscr()[32 - 1] = n;
@@ -1689,7 +1667,7 @@ FE_FN void fe_solve_coop(FeWarp* w) {
   LANES_END
   const int nA = w->iscr()[31];
   bool regs = nA <= 32;
-  if (!fast) for (int p = 0; p < m->npart; ++p) if (w->plist()[9 * p + 8] > 8) regs = false; // needs the grouped static-contact path
+  for (int p = 0; p < np; ++p) if (w->plist()[9 * p + 8] > 8) regs = false; // needs the grouped static-contact path
   int iter = 0;
   float cost = 0.f, impr = 0.f;
   FE_TICK(w->u() + FE_U_STAT, FE_STAT_NEWTON_SETUP) // this solver's phases in the FE_STAT_NEWTON_* columns: include/furniture_b200.h
@@ -1719,18 +1697,17 @@ FE_FN void fe_solve_coop(FeWarp* w) {
     FE_TICK(w->u() + FE_U_STAT, FE_STAT_NEWTON_HESSIAN)
     if (regs) {
       LANES_BEGIN for (int i = lane; i < nv; i += 32) w->search()[i] = -w->grad()[i]; LANES_END
-      if (!fast) { fe_chol_blocks(w, w->H(), w->skip()); fe_solve_blocks(w, w->H(), w->skip(), w->search()); }
+      fe_chol_blocks(w, w->H(), w->skip());
+      fe_solve_blocks(w, w->H(), w->skip(), w->search());
       FE_TICK(w->u() + FE_U_STAT, FE_STAT_NEWTON_CHOL)
       if (nA <= 16) fe_newton_regs<16>(w, nA); else if (nA <= 24) fe_newton_regs<24>(w, nA); else fe_newton_regs<32>(w, nA);
     } else {
-      const int* skip = nullptr;
-      if (!fast) { // FULL scope: independent part blocks are factored / solved by one lane each
-        fe_mark_indep_blocks(w, w->first(), w->skip());
-        fe_chol_blocks(w, w->H(), w->skip());
-        skip = w->skip();
-      }
+      // independent part blocks are factored / solved by one lane each
+      const int* skip = w->skip();
+      fe_mark_indep_blocks(w, w->first(), w->skip());
+      fe_chol_blocks(w, w->H(), skip);
       LANES_BEGIN for (int i = lane; i < nv; i += 32) w->search()[i] = -w->grad()[i]; LANES_END
-      if (skip) fe_solve_blocks(w, w->H(), skip, w->search());
+      fe_solve_blocks(w, w->H(), skip, w->search());
       if (!fe_chol(w, w->H(), w->first(), nv, skip)) { LANES_BEGIN if (lane == 0) w->u()[FE_U_FLAGS] |= FE_FLAG_NEWTON_PIVOT; LANES_END }
       FE_TICK(w->u() + FE_U_STAT, FE_STAT_NEWTON_CHOL)
       fe_chol_solve(w, w->H(), w->first(), nv, w->search(), w->Mv(), skip);
@@ -1758,10 +1735,8 @@ FE_FN void fe_solve_coop(FeWarp* w) {
     impr = ls.impr();
     LANES_BEGIN
       for (int i = lane; i < nv; i += 32) { w->x()[i] += alpha * w->search()[i]; w->Ma()[i] += alpha * w->Mv()[i]; }
-      for (int c = lane; c < ncon; c += 32) {
-        if (fast && w->c_kind()[c] == 0) continue;
+      for (int c = lane; c < ncon; c += 32)
         for (int k = 0; k < 3; ++k) w->c_jar()[3 * c + k] += alpha * w->c_jv()[3 * c + k];
-      }
       for (int e = lane; e < 6 * ne; e += 32) w->w_jar()[e] += alpha * w->w_jv()[e];
       for (int d = lane; d < nr; d += 32) w->l_jar()[d] += alpha * w->l_jv()[d];
     LANES_END
@@ -1776,15 +1751,12 @@ FE_FN void fe_solve_coop(FeWarp* w) {
   FE_TICK(w->u() + FE_U_STAT, FE_STAT_NEWTON_SETUP)
 }
 
-
-// ---- single-lane Newton solve of one free part whose contacts are all against the static world (FAST scope).
-// Same cost, cones and exact line search as the cooperative solver, on the part's own 6 unknowns [alpha; vdot]; the
-// blocks are independent in that case, so block-wise Newton converges to the same minimiser as MuJoCo's global iteration.
-// FAST scope, free parts: 8 lanes per part (4 parts per pass), one lane per contact.  Per Newton iteration each lane
-// evaluates its contact (cone zone, force, 3x3 weight, J^T f and J^T W J), the group sums them with 3 xor-shuffles per
-// value, every lane of the group then factors the same 6x6 Hessian and runs the same exact line search, whose
-// per-contact terms are again group-summed.  Parts are independent blocks here, so block-wise Newton reaches the same
-// minimiser as the global iteration.
+// ---- free parts whose contacts are all against the static world (the parts in skipmask are left out), on each part's own
+// 6 unknowns [alpha; vdot] with the cost, cones and exact line search of the cooperative solver.  8 lanes per part (4 parts
+// per pass), one lane per contact.  Per Newton iteration each lane evaluates its contact (cone zone, force, 3x3 weight,
+// J^T f and J^T W J), the group sums them with 3 xor-shuffles per value, every lane of the group then factors the same 6x6
+// Hessian and runs the same exact line search, whose per-contact terms are again group-summed.  Parts are independent
+// blocks here, so block-wise Newton reaches the same minimiser as the global iteration.
 FE_FN void fe_solve_parts_grouped(FeWarp* w, unsigned skipmask) {
   const fe_model* m = w->m;
   const int nr = m->nr, nrl = m->nrlink, np = m->npart, maxit = w->opt.newton_iters, maxls = w->opt.ls_iters;
@@ -1983,7 +1955,7 @@ FE_FN void fe_solve_parts_grouped(FeWarp* w, unsigned skipmask) {
   }
 }
 
-// ---- FAST scope, robot block whose only constraint rows are joint limits (no robot contact): the common case, e.g. the
+// ---- robot block whose only constraint rows are joint limits (no robot contact): the common case, e.g. the
 // gripper fingers resting on their stops.  Lane d owns dof d in registers; M products are 9 shuffles + 9 FMAs per lane,
 // reductions are xor-butterflies, only the small Cholesky goes through the slice.  Same cost function as fe_solve_coop, with
 // the stop test fe_newton_stop and the exact line search FeLineSearch that every Newton solver here uses.
@@ -2077,6 +2049,19 @@ FE_FN void fe_solve_robot_limits(FeWarp* w) {
 
 #include "fe_solve_comp.h"
 
+// fe_solve_parts_grouped over the parts not in skipmask; their largest iteration count goes to FE_U_NITER and is added to
+// the FE_STAT_PART_ITERS column
+FE_HD void fe_solve_free_parts(FeWarp* w, unsigned skipmask) {
+  fe_solve_parts_grouped(w, skipmask);
+  LANES_BEGIN
+    if (lane == 0) {
+      int mx = 0;
+      for (int p = 0; p < w->m->npart; ++p) if (!((skipmask >> p) & 1u)) mx = w->iscr()[p] > mx ? w->iscr()[p] : mx;
+      w->u()[FE_U_NITER] = mx; w->u()[FE_U_STAT + FE_STAT_PART_ITERS] += mx;
+    }
+  LANES_END
+}
+
 // mj_fwdConstraint.  The constraint set of this mj_step is split into independent pieces (the cost is separable over them):
 // free parts that only touch the static world (8 lanes per part, fe_solve_parts_grouped), the robot block when its only
 // rows are joint limits (fe_solve_robot_limits), and the coupled component -- robot block with contacts, parts in contact
@@ -2109,10 +2094,7 @@ FE_FN void fe_solve(FeWarp* w) {
   const unsigned cplmask = fe_ballot32(w->iscr());
   const bool robot_in = fe_ballot32(w->colmap()) != 0u;
   if (cplmask == 0u && !robot_in) { // nothing couples two moving blocks and the robot touches nothing
-    fe_solve_parts_grouped(w, 0u);
-    LANES_BEGIN
-      if (lane == 0) { int mx = 0; for (int p = 0; p < np; ++p) mx = w->iscr()[p] > mx ? w->iscr()[p] : mx; w->u()[FE_U_NITER] = mx; w->u()[FE_U_STAT + FE_STAT_PART_ITERS] += mx; }
-    LANES_END
+    fe_solve_free_parts(w, 0u);
     fe_solve_robot_limits(w);
     return;
   }
@@ -2149,10 +2131,7 @@ FE_FN void fe_solve(FeWarp* w) {
   }
   if (nA <= 32 && ncc <= 32) {
     FE_TICK(w->u() + FE_U_STAT, FE_STAT_SOLVE_PRE)
-    fe_solve_parts_grouped(w, cplmask);
-    LANES_BEGIN
-      if (lane == 0) { int mx = 0; for (int p = 0; p < np; ++p) if (!((cplmask >> p) & 1u)) mx = w->iscr()[p] > mx ? w->iscr()[p] : mx; w->u()[FE_U_NITER] = mx; w->u()[FE_U_STAT + FE_STAT_PART_ITERS] += mx; }
-    LANES_END
+    fe_solve_free_parts(w, cplmask);
     if (!robot_in) fe_solve_robot_limits(w);
     FE_TICK(w->u() + FE_U_STAT, FE_STAT_SOLVE_GROUPED)
     if (nA <= 16) fe_solve_comp<16>(w, nA, ncc, cplmask, robot_in ? 1 : 0);
@@ -2161,17 +2140,7 @@ FE_FN void fe_solve(FeWarp* w) {
     FE_TICK(w->u() + FE_U_STAT, FE_STAT_SOLVE_COMP)
     return;
   }
-  // fallback: cooperative solver in shared memory (all dofs when something couples, else the robot block)
-  const bool coupled = cplmask != 0u;
-  LANES_BEGIN if (lane == 0) { w->fast = coupled ? 0 : 1; w->nact = coupled ? m->nv : m->nr; } LANES_END
-  if (!coupled) {
-    fe_solve_parts_grouped(w, 0u);
-    LANES_BEGIN
-      if (lane == 0) { int mx = 0; for (int p = 0; p < np; ++p) mx = w->iscr()[p] > mx ? w->iscr()[p] : mx; w->u()[FE_U_NITER] = mx; w->u()[FE_U_STAT + FE_STAT_PART_ITERS] += mx; }
-    LANES_END
-  }
-  fe_solve_coop(w);
-  LANES_BEGIN if (lane == 0) { w->fast = 0; w->nact = m->nv; } LANES_END
+  fe_solve_coop(w, cplmask); // fallback: the cooperative solver in shared memory, over all dofs
 }
 
 // ---------------------------------------------------------------- mj_Euler + mj_advance

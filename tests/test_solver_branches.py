@@ -6,8 +6,9 @@ fe_solve splits the constraint set of one mj_step into pieces and sends each to 
   robot limits   fe_solve_robot_limits: the robot block when its only rows are joint limits
   comp<16|24|32> fe_solve_comp: the coupled component (robot with contacts, parts touching the robot or each other, welded
                  parts) when it has nA <= 32 dofs and ncc <= 32 contacts; the template is picked by nA
-  coop           fe_solve_coop beyond that: the register Newton direction fe_newton_regs when its own active set has <= 32
-                 dofs and no part has more than 8 static contacts, else the shared-memory fe_chol / fe_chol_solve
+  coop           fe_solve_coop beyond that, over all dofs: the register Newton direction fe_newton_regs when the robot block
+                 and the coupled parts have <= 32 dofs and no part has more than 8 static contacts, else the shared-memory
+                 fe_chol / fe_chol_solve
 `classify` restates that rule on the oracle's contact list, so that every state says which branch it is meant to reach and
 the coverage table below is asserted, not assumed.
 
@@ -23,7 +24,7 @@ import numpy as np
 import pytest
 
 from furniture_b200 import mjcf
-from furniture_b200.engine import FLAG_CONTACT_FULL
+from furniture_b200.engine import FLAG_CONTACT_FULL, auto_maxcon
 from furniture_b200.engine_model import EngineModel
 from oracle.assembly_oracle import rel_pose
 from oracle.oracle import OracleSim
@@ -68,7 +69,7 @@ def classify(m, em, contacts, eq_active):
     cpl = [touch[p] or welded[p] or nstat[p] > 8 for p in range(npart)]
     nA = (nr if robot_in else 0) + 6 * sum(cpl)
     ncc = sum(1 for k, p in zip(kinds, owner) if k != 0 or cpl[p])
-    info = dict(nA=nA, ncc=ncc, nstat=nstat, robot_in=robot_in, weld=any(welded), ncon=len(contacts))
+    info = dict(nA=nA, ncc=ncc, ncpl=sum(cpl), nstat=nstat, robot_in=robot_in, weld=any(welded), ncon=len(contacts))
     if not any(cpl) and not robot_in:
         units, passes, p0 = [], 0, 0
         while p0 < npart:  # fe_solve_parts_grouped's packing: 8 units of 4 lanes per pass, a wide part on an aligned pair
@@ -84,8 +85,8 @@ def classify(m, em, contacts, eq_active):
         return dict(info, branch="grouped", passes=passes)
     if nA <= 32 and ncc <= 32:
         return dict(info, branch="comp%d" % (16 if nA <= 16 else 24 if nA <= 24 else 32))
-    # fe_solve_coop: its register active set is the robot block plus every part coupled by a kind 2 / 3 contact, a weld or
-    # more than 8 static contacts; a part with more than 8 static contacts also sends the direction to the Cholesky path
+    # fe_solve_coop: its register active set is the robot block plus the coupled parts; a part with more than 8 static
+    # contacts also sends the direction to the Cholesky path
     nreg = nr + 6 * sum(cpl)
     regs = nreg <= 32 and max(nstat, default=0) <= 8
     return dict(info, branch="coop_regs" if regs else "coop_chol")
@@ -102,6 +103,12 @@ def _near_activation(m, em, probe, q, eqa, eqd, oc):
     probe.qpos[:] = q; probe.eq_active[:] = eqa; probe.eq_data[:] = eqd
     probe.stage("kinematics"); probe.stage("collision")
     return sum(map(on_part, probe.contacts())) != sum(map(on_part, oc))
+
+
+def _mpr(m, contacts):
+    """a contact that the narrow phase finds with MPR: a cylinder against anything but a plane, or a mesh"""
+    types = [(m.geom_type[c.geom1], m.geom_type[c.geom2]) for c in contacts]
+    return any(GEOM_CYLINDER in t and 0 not in t or GEOM_MESH in t for t in types)
 
 
 @functools.lru_cache(maxsize=None)
@@ -144,9 +151,7 @@ def pile_states(name, npile, seed, weld_every=0, spread=0.05, away=0.0):
             oc = sim.contacts()
             if _near_activation(m, em, probe, q_, eqa, eqd.ravel(), oc):
                 continue
-            mpr = any(GEOM_CYLINDER in (m.geom_type[c.geom1], m.geom_type[c.geom2]) and 0 not in (m.geom_type[c.geom1], m.geom_type[c.geom2])
-                      or GEOM_MESH in (m.geom_type[c.geom1], m.geom_type[c.geom2]) for c in oc)
-            out.append(dict(qpos=q_, qvel=v_, warm=w_, eq_active=eqa.copy(), eq_data=eqd.ravel().copy(), mpr=mpr, nl=sim.solver_info()["nl"],
+            out.append(dict(qpos=q_, qvel=v_, warm=w_, eq_active=eqa.copy(), eq_data=eqd.ravel().copy(), mpr=_mpr(m, oc), nl=sim.solver_info()["nl"],
                             **classify(m, em, oc, eqa)))
     return m, em, out
 
@@ -186,6 +191,9 @@ ROWS = {
     "coop, Cholesky: nA 33": ("lack", lambda s: s["branch"] == "coop_chol" and s["nA"] == 33, 3),
     "coop, Cholesky: nA 39": ("lack_weld", lambda s: s["branch"] == "coop_chol" and s["nA"] == 39, 3),
     "coop, Cholesky: part with > 8 static contacts": ("ingolf+ingolf2", lambda s: s["branch"] == "coop_chol" and max(s["nstat"]) > 8, 3),
+    # the robot block with more than 32 contacts of its own and no coupled part: the free parts are independent blocks of
+    # the cooperative solve
+    "coop, robot block only": ("floor", lambda s: s["branch"] == "coop_regs" and s["ncpl"] == 0 and s["ncc"] > 32, 3),
 }
 
 
@@ -208,9 +216,41 @@ def limit_states():
     return m, em, out
 
 
+# Sawyer joint angles (7 arm joints, 2 fingers) that press the gripper, wrist and forearm into the floor: 33 contacts, every
+# one against the floor and at most 5 cm deep.  Found by a seeded random search over the joint ranges; only forward() and one
+# mj_step are run from them, so they need not be reachable.
+FLOOR_POSES = [
+    [1.0938, -3.7266, -3.5843, 1.1069, -2.5768, 1.134, 1.8143, 0.0024, -0.0089],
+    [-1.118, 0.8512, -3.4275, 0.3658, 0.1351, -2.4323, -1.5418, 0.0088, 0.0087],
+]
+
+
+@functools.lru_cache(maxsize=None)
+def floor_states():
+    """grouped states of the pile source in which every part rests on the floor, with the arm set to each of FLOOR_POSES"""
+    m, em, states = pile_states(*SOURCES["lack"])
+    sim, probe = OracleSim(m), OracleSim(m)
+    probe.set_model("geom_margin", np.asarray(m.a["geom_margin"], np.float64) + NEAR)
+    out = []
+    for s in states:
+        if s["branch"] != "grouped" or min(s["nstat"]) == 0:
+            continue
+        for arm in FLOOR_POSES:
+            q = s["qpos"].copy()
+            q[: len(arm)] = arm
+            sim.qpos[:] = q; sim.qvel[:] = s["qvel"]; sim.qacc_warmstart[:] = s["warm"]; sim.eq_active[:] = s["eq_active"]; sim.eq_data[:] = s["eq_data"]
+            sim.forward()
+            oc = sim.contacts()
+            if _near_activation(m, em, probe, q, s["eq_active"], s["eq_data"], oc):
+                continue
+            out.append(dict(s, qpos=q, mpr=_mpr(m, oc), nl=sim.solver_info()["nl"], **classify(m, em, oc, s["eq_active"])))
+    return m, em, out
+
+
 def source(names):
     """the states of one source, or of several joined by '+' (same model)"""
-    got = [limit_states() if n == "limits" else pile_states(*SOURCES[n]) for n in names.split("+")]
+    built = {"limits": limit_states, "floor": floor_states}
+    got = [built[n]() if n in built else pile_states(*SOURCES[n]) for n in names.split("+")]
     return got[0][0], got[0][1], [s for g in got for s in g[2]]
 
 
@@ -286,7 +326,8 @@ def test_every_dispatch_branch_matches_oracle(gpu):
         by_model.setdefault(m.meta["furniture_name"] if "furniture_name" in m.meta else id(m), (m, em, []))[2].extend((row, s) for s in states)
     for m, em, rs in by_model.values():
         states = [s for _, s in rs]
-        eng = make_engine(m, len(states), gpu)
+        # room for every contact: the arm pressed into the floor next to resting parts has more than the scene's default
+        eng = make_engine(m, len(states), gpu, maxcon=max(auto_maxcon(em), max(s["ncon"] for s in states)))
         sims = _check_forward(m, em, eng, states, rs[0][0])
         eng.step(1)
         qe, ve = eng.get("qpos"), eng.get("qvel")
