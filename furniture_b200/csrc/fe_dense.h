@@ -1,6 +1,6 @@
 // fe_dense.h -- the phase-based dense reward of FurnitureSawyerDenseRewardEnv, evaluated by lane 0 of the warp that owns the env
 // right after the physics of the step (furniture/env/furniture_sawyer_dense.py):
-//   fe_dense_begin_episode <- _reset_reward_variables :128-139 (no preassembled parts)
+//   fe_dense_begin_episode <- _reset_reward_variables :128-139
 //   fe_dense_begin_subtask <- _update_reward_variables :150-219, _set_next_subtask :141-148
 //   fe_dense_step          <- _collect_values :225-280, _compute_reward :282-586, the eight phase terms :588-943,
 //                             _stable_grip_reward :945-985, _gripper_penalty :987-1003, _ctrl_penalty :1005-1009,
@@ -62,9 +62,11 @@ FE_HDN void fe_dense_begin_subtask(const W& w, const fe_dense_config* c, const f
   }
 }
 
+// `first`: the subtask the episode starts at, the number of recipe steps the reset preassembled.  Their legs' grasp-target pairs are claimed in
+// recipe order (:130-138), which is the order the packed gl_site / gr_site were resolved in: subtask `first` holds the pair it would claim.
 template <class W>
-FE_HDN void fe_dense_begin_episode(const W& w, const fe_dense_config* c, const fe_dense_recipe* rc, FeDenseState* st) {
-  st->subtask = 0;
+FE_HDN void fe_dense_begin_episode(const W& w, const fe_dense_config* c, const fe_dense_recipe* rc, int first, FeDenseState* st) {
+  st->subtask = first;
   st->success = 0;
   for (int k = 0; k < FE_DP_N; ++k) st->prev[k] = 0.0;
   st->prev[FE_DP_GRASP] = -1.0;
@@ -108,15 +110,8 @@ FE_HDN void fe_dense_step(const W& w, const fe_dense_config* c, const fe_dense_r
     double k[3], cr[3];
     np_unit_vector_f32(k, leg_up);
     npcross(cr, k, leg_fw);
-    if (rc->has_angle[s]) {
-      for (int i = 0; i < 3; ++i) fw_rot[i] = ndadd(ndmul(rc->angle_cos[s], leg_fw[i]), ndmul(rc->angle_sin[s], cr[i]));
-    } else {
-      const double cs = np_cos_siml(leg_fw, table_fw), sn = ndsqrt(ndsub(1.0, ndmul(cs, cs)));
-      double fp[3], fn[3];
-      for (int i = 0; i < 3; ++i) { fp[i] = ndadd(ndmul(cs, leg_fw[i]), ndmul(ndmul(1.0, sn), cr[i])); fn[i] = ndadd(ndmul(cs, leg_fw[i]), ndmul(ndmul(-1.0, sn), cr[i])); }
-      const bool plus = np_cos_siml(fp, table_fw) > np_cos_siml(fn, table_fw);
-      for (int i = 0; i < 3; ++i) fw_rot[i] = plus ? fp[i] : fn[i];
-    }
+    if (rc->has_angle[s]) for (int i = 0; i < 3; ++i) fw_rot[i] = ndadd(ndmul(rc->angle_cos[s], leg_fw[i]), ndmul(rc->angle_sin[s], cr[i]));
+    else np_rotate_towards(fw_rot, leg_fw, cr, table_fw);
   } else {
     for (int i = 0; i < 3; ++i) fw_rot[i] = leg_fw[i];
   }
@@ -298,7 +293,7 @@ struct FeArrayWorld {
   FE_MEMBER bool touch_both(int q) const { return touch[q] != 0; }
 };
 
-// one thread walks the records of one episode: a record with reset != 0 starts the episode on the world it shows
+// one thread walks the records of one episode: a record with reset != 0 starts the episode on the world it shows, at subtask reset - 1
 FE_HDN void fe_dense_eval_episode(const fe_dense_config* c, const fe_dense_recipe* rc, const double* thr, int n_goal, int first, int count, int nsite, int npart,
                                   int act_dim, const double* spos, const double* smat, const double* ppos, const uint8_t* touch, const uint8_t* reset,
                                   const uint8_t* connected, const double* ac, double* reward, uint8_t* done, double* info) {
@@ -307,7 +302,7 @@ FE_HDN void fe_dense_eval_episode(const fe_dense_config* c, const fe_dense_recip
     FeArrayWorld w = {spos + (size_t)t * nsite * 3, smat + (size_t)t * nsite * 9, ppos + (size_t)t * npart * 3, touch + (size_t)t * npart};
     double* inf = info + (size_t)t * FE_DENSE_INFO;
     if (reset[t]) {
-      fe_dense_begin_episode(w, c, rc, &st);
+      fe_dense_begin_episode(w, c, rc, reset[t] - 1, &st);
       reward[t] = 0.0; done[t] = 0;
       for (int k = 0; k < FE_DENSE_INFO; ++k) inf[k] = 0.0;
       inf[0] = (double)st.phase; inf[1] = (double)st.subtask;

@@ -45,6 +45,8 @@ struct FeEnvState {
                                                // the send buffer of the multi-GPU all-gather, written by the step kernel itself
   int *group, *site_connected;                 // [N][npart], [N][nsite]
   int *num_connected, *prev_num_connected, *touched, *picked, *episode_len, *done;
+  int *preassembled, *num_connects;            // [N] set_subtask (furniture.py:204-207): recipe steps connected by the env's next reset; connections asked for, -1 = None
+  int* success_num_conn;                       // [N] _success_num_conn as the env's last reset left it (furniture.py:1477-1481)
   uint32_t* mt;                                // [N][624] MT19937 state of the env's numpy RandomState(seed + env)
   int* mt_pos;                                 // [N] position in the state (624 = regenerate before the next draw)
   int *robot_contype, *robot_conaff;           // [N][ngeom] saved robot masks during reset
@@ -117,6 +119,15 @@ FE_HDN void np_lookat_wxyz(double* out, const double* forward, const double* up)
   }
   out[0] = q[3]; out[1] = q[0]; out[2] = q[1]; out[3] = q[2];
 }
+// the better of transform_utils.rotate_vector_cos_siml(f1, up1, cos_siml(f1, f2), +-1) by cos_siml with f2; cr = cross(unit_vector(up1), f1)
+FE_HD void np_rotate_towards(double* fr, const double* f1, const double* cr, const double* f2) {
+  const double c = np_cos_siml(f1, f2);
+  const double s = ndsqrt(ndsub(1.0, ndmul(c, c)));
+  double fp[3], fn[3];
+  for (int i = 0; i < 3; ++i) { fp[i] = ndadd(ndmul(c, f1[i]), ndmul(ndmul(1.0, s), cr[i])); fn[i] = ndadd(ndmul(c, f1[i]), ndmul(ndmul(-1.0, s), cr[i])); }
+  const bool pos = np_cos_siml(fp, f2) > np_cos_siml(fn, f2);
+  for (int i = 0; i < 3; ++i) fr[i] = pos ? fp[i] : fn[i];
+}
 // FurnitureEnv._is_aligned (furniture.py:1057-1153). m*: row-major site rotation. cs/sn: cos/sin of the allowed angles.
 // Returns the decision; *tq_set tells whether _target_connector_xquat was assigned, tq its value (wxyz).
 FE_HDN bool fe_is_aligned_d(const double* p1, const double* m1, const double* p2, const double* m2, int nang, const double* cs, const double* sn,
@@ -137,12 +148,7 @@ FE_HDN bool fe_is_aligned_d(const double* p1, const double* m1, const double* p2
   npcross(cr, k, f1);
   if (nang == 0) {
     fwd_ok = true;
-    const double c = np_cos_siml(f1, f2);
-    const double s = ndsqrt(ndsub(1.0, ndmul(c, c)));
-    double fp[3], fn[3];
-    for (int i = 0; i < 3; ++i) { fp[i] = ndadd(ndmul(c, f1[i]), ndmul(ndmul(1.0, s), cr[i])); fn[i] = ndadd(ndmul(c, f1[i]), ndmul(ndmul(-1.0, s), cr[i])); }
-    const bool pos = np_cos_siml(fp, f2) > np_cos_siml(fn, f2);
-    for (int i = 0; i < 3; ++i) fr[i] = pos ? fp[i] : fn[i];
+    np_rotate_towards(fr, f1, cr, f2);
     np_lookat_wxyz(tq, up1, fr);
     *tq_set = true;
   } else {
@@ -159,6 +165,17 @@ FE_HDN bool fe_is_aligned_d(const double* p1, const double* m1, const double* p2
   if (pos_dist < thr[0] && rot_up > thr[1] && fwd_ok && fabs(proj12) > thr[3] && fabs(proj21) > thr[3]) return true;
   if (pos_dist < nddiv(thr[0], 2.0) && rot_up > thr[1] && fwd_ok) return true;
   return false;
+}
+// FurnitureEnv._project_connector_quat(connector1, connector2, angle) (furniture.py:1201-1222): connector2's xquat (wxyz) when aligned with
+// connector1.  m*: row-major site rotation; cs / sn: cos / sin of the recipe angle when it gives one.
+FE_HDN void fe_project_connector_quat_d(const double* m1, const double* m2, int has_angle, double cs, double sn, double* tq) {
+  const double up1[3] = {m1[2], m1[5], m1[8]}, f1[3] = {m1[1], m1[4], m1[7]}, f2[3] = {m2[1], m2[4], m2[7]};
+  double k[3], cr[3], fr[3];
+  np_unit_vector_f32(k, up1);
+  npcross(cr, k, f1);
+  if (has_angle) for (int i = 0; i < 3; ++i) fr[i] = ndadd(ndmul(cs, f1[i]), ndmul(sn, cr[i]));
+  else np_rotate_towards(fr, f1, cr, f2);
+  np_lookat_wxyz(tq, up1, fr);
 }
 
 #include "fe_dense.h"
@@ -228,7 +245,7 @@ struct FeEnvScratchD {
   double lift;           // lowest site z of the two connected groups (floor clearance)
 };
 struct FeEnvScratchI {
-  int aligned;           // fe_try_connect_scan found an aligned pair
+  int aligned;           // fe_try_connect_scan found an aligned pair and no reset has followed: _connected, a connection made during this step
   int repin;             // part to re-pin at body1_pose after the step (_connected_body1), -1 = none
   int site1, site2;      // sites of the aligned pair
   int conn1, conn2;      // their connector indices
@@ -354,8 +371,9 @@ FE_FN void fe_try_connect_scan(FeEnv* e, int part1) {
   LANES_END
 }
 
-// _connect(site1, site2) (furniture.py:847-924) for arm agents
-FE_FN void fe_connect(FeEnv* e) {
+// _connect(site1, site2, auto_align) (furniture.py:847-924) for arm agents: the pair in si->site1 .. conn2, its target quat in sd->target_quat.
+// `force_align`: align the connectors whatever cfg->auto_align says (the reset's preassembly, furniture.py:1556)
+FE_FN void fe_connect(FeEnv* e, bool force_align) {
   FeWarp* w = e->w;
   const fe_model* m = w->m;
   const fe_scene* sc = e->sc;
@@ -371,7 +389,7 @@ FE_FN void fe_connect(FeEnv* e) {
         const int gp = fe_find(e->group, p);
         if ((gp == g1 || gp == g2) && w->contype()[g] != 0) { w->contype()[g] = (1 << 30) - 1 - (1 << (g1 + 1)); w->conaff()[g] = 1 << (g1 + 1); }
       }
-      if (e->cfg->auto_align) { // _align_connectors -> _move_site_to_target (furniture.py:1224-1250)
+      if (e->cfg->auto_align || force_align) { // _align_connectors -> _move_site_to_target (furniture.py:1224-1250)
         double target[7], base[7], sp[3], sq[4];
         fe_site_pose_d(w, s1, sp, nullptr, sq);
         for (int k = 0; k < 3; ++k) target[k] = sp[k];
@@ -495,8 +513,47 @@ FE_FN void fe_write_obs(FeEnv* e) {
   }
 }
 
-// FurnitureEnv._reset (furniture.py:1406-1663); the warp slice is (re)initialised here, caller stores it
-FE_FN void fe_env_reset_one(FeEnv* e) {
+// stabilise furniture: 10 x { stop(gravity=0); 10 x { forward; step; slow } }  (furniture.py:1535-1540, :1560-1566)
+FE_FN void fe_env_stabilise(FeEnv* e) {
+  FeWarp* w = e->w;
+  const fe_model* m = w->m;
+  const int nrl = m->nrlink, np = m->npart;
+  for (int outer = 0; outer < 10; ++outer) {
+    LANES_BEGIN for (int p = lane; p < np; p += 32) fe_stop_part(w, p, 0.f); LANES_END
+    for (int inner = 0; inner < 10; ++inner) {
+      fe_fwd_step(e);
+      LANES_BEGIN
+        for (int p = lane; p < np; p += 32) { // _slow_object: full gravity compensation + velocity clip (furniture.py:2821-2842)
+          const int da = m->link_dadr[nrl + p];
+          w->gravcomp()[p] = 1.f;
+          for (int k = 0; k < 6; ++k) w->qvel()[da + k] = fminf(fmaxf(w->qvel()[da + k], -0.2f), 0.2f);
+        }
+      LANES_END
+    }
+  }
+}
+
+// the pair and the target of the preassembly's i-th connection (furniture.py:1544-1555), left where fe_try_connect_scan leaves an aligned pair.
+// _connect(site2_id, site1_id): the table's connector is _connect's site1, so the leg's group is moved onto the table.
+FE_FN void fe_env_preassemble_pair(FeEnv* e, int i) {
+  const fe_scene* sc = e->sc;
+  const fe_dense_recipe* rc = &sc->dense;
+  LANES_BEGIN
+    if (lane == 0) {
+      const int s1 = rc->table_site[i], s2 = rc->leg_site[i];
+      double p[3], m1[9], m2[9];
+      fe_site_pose_d(e->w, s1, p, m1, nullptr);
+      fe_site_pose_d(e->w, s2, p, m2, nullptr);
+      fe_project_connector_quat_d(m1, m2, rc->has_angle[i], rc->angle_cos[i], rc->angle_sin[i], e->sd->target_quat);
+      e->si->site1 = s1; e->si->site2 = s2;
+      for (int c = 0; c < sc->nconn; ++c) { if (sc->conn_site[c] == s1) e->si->conn1 = c; if (sc->conn_site[c] == s2) e->si->conn2 = c; }
+    }
+  LANES_END
+}
+
+// FurnitureEnv._reset (furniture.py:1406-1663) in two calls with the preassembly between them (fe_env_reset_one), so that its connect path does
+// not stack on their frames: up to the furniture at rest, with `pre` recipe steps to preassemble, and from the robot's pose on
+FE_FN void fe_env_reset_furniture(FeEnv* e, int pre) {
   FeWarp* w = e->w;
   const fe_model* m = w->m;
   const fe_scene* sc = e->sc;
@@ -520,6 +577,9 @@ FE_FN void fe_env_reset_one(FeEnv* e) {
     for (int s = lane; s < m->nsite; s += 32) e->es.site_connected[(size_t)e->env * m->nsite + s] = 0;
     if (lane == 0) {
       e->es.num_connected[e->env] = 0; e->es.prev_num_connected[e->env] = 0; e->es.episode_len[e->env] = 0; e->es.episode_reward[e->env] = 0.f;
+      const int ask = e->es.num_connects[e->env];
+      e->es.success_num_conn[e->env] = ask >= 0 ? ask + pre : np - 1; // furniture.py:1477-1481
+      e->si->aligned = 0;                                             // _connected = False (:1468)
       w->u()[FE_U_FLAGS] = 0;
     }
   LANES_END
@@ -555,20 +615,16 @@ FE_FN void fe_env_reset_one(FeEnv* e) {
       e->es.mt_pos[e->env] = pos;
     }
   LANES_END
-  // stabilise furniture: 10 x { stop(gravity=0); 10 x { forward; step; slow } }  (furniture.py:1535-1540)
-  for (int outer = 0; outer < 10; ++outer) {
-    LANES_BEGIN for (int p = lane; p < np; p += 32) fe_stop_part(w, p, 0.f); LANES_END
-    for (int inner = 0; inner < 10; ++inner) {
-      fe_fwd_step(e);
-      LANES_BEGIN
-        for (int p = lane; p < np; p += 32) { // _slow_object: full gravity compensation + velocity clip (furniture.py:2821-2842)
-          const int da = m->link_dadr[nrl + p];
-          w->gravcomp()[p] = 1.f;
-          for (int k = 0; k < 6; ++k) w->qvel()[da + k] = fminf(fmaxf(w->qvel()[da + k], -0.2f), 0.2f);
-        }
-      LANES_END
-    }
-  }
+  fe_env_stabilise(e);
+}
+FE_FN void fe_env_reset_robot(FeEnv* e, int pre) {
+  FeWarp* w = e->w;
+  const fe_model* m = w->m;
+  const fe_scene* sc = e->sc;
+  const fe_config* cfg = e->cfg;
+  const int nr = m->nr, np = m->npart, ng = m->ngeom;
+  const int* rct = e->es.robot_contype + (size_t)e->env * ng;
+  const int* rca = e->es.robot_conaff + (size_t)e->env * ng;
   // gravity compensation, robot pose, one step with robot collisions still off (furniture.py:1569-1584)
   for (int phase = 0; phase < 101; ++phase) {
     LANES_BEGIN
@@ -604,13 +660,24 @@ FE_FN void fe_env_reset_one(FeEnv* e) {
   LANES_BEGIN
     if (lane == 0) {
       e->es.done[e->env] = 0;
+      e->si->repin = -1; // _connected_body1 = None (:1558): the preassembly leaves no re-pin pending
       if (e->es.dense) { // FurnitureSawyerDenseRewardEnv._reset: _reset_reward_variables on the settled scene
         FeSliceWorld world = {w};
-        fe_dense_begin_episode(world, e->es.dense, &sc->dense, e->es.dstate + e->env); // dense_info keeps the last step's terms (the terminal step's, after an auto-reset)
+        fe_dense_begin_episode(world, e->es.dense, &sc->dense, pre, e->es.dstate + e->env); // dense_info keeps the last step's terms (the terminal step's, after an auto-reset)
       }
     }
   LANES_END
   fe_write_obs(e);
+}
+// the warp slice is (re)initialised here, caller stores it
+FE_FN void fe_env_reset_one(FeEnv* e) {
+  const fe_scene* sc = e->sc;
+  const int want = e->es.preassembled[e->env], cap = sc->dense.nsub - (e->es.dense && sc->dense.nsub > 0 ? 1 : 0); // a recipe prefix; the dense reward needs a subtask left
+  const int pre = want < 0 ? 0 : (want > cap ? cap : want);
+  fe_env_reset_furniture(e, pre);
+  for (int i = 0; i < pre; ++i) { fe_env_preassemble_pair(e, i); fe_connect(e, true); } // :1542-1558, robot collisions still off
+  if (pre > 0) fe_env_stabilise(e);                                                      // :1560-1566
+  fe_env_reset_robot(e, pre);
 }
 
 // the per-step flags: no connection found, no re-pin pending, no auto-reset due, no simulation failure yet (lane 0)
@@ -659,7 +726,7 @@ FE_HD void fe_env_finish(FeEnv* e, const float* a, int act_dim, float connect, i
         for (int p = 0; p < np; ++p) if ((w->touch()[p] & both) == both) { part = p; break; }
         if (part >= 0) {
           fe_try_connect_scan(e, part);
-          if (e->si->aligned) { fe_connect(e); break; }
+          if (e->si->aligned) { fe_connect(e, false); break; }
         }
       }
     }
@@ -695,12 +762,13 @@ FE_HD void fe_env_finish(FeEnv* e, const float* a, int act_dim, float connect, i
           }
       const int nc = e->es.num_connected[env];
       const float success_r = cfg->success_reward * (float)(nc - e->es.prev_num_connected[env]);
-      const int connected_now = nc != e->es.prev_num_connected[env]; // _connected: a connection was made during this step
+      const int connected_now = e->si->aligned; // _connected: a connection was made during this step (the legs a reset preassembles are not one)
       e->es.prev_num_connected[env] = nc;
       float sq = 0.f;
       for (int k = 0; k < act_dim; ++k) sq += a[k] * a[k];
       float reward = success_r + touch_r + pick_r - cfg->ctrl_penalty_coef * sq;
-      int success = (nc == np - 1 && np > 1) ? 1 : 0;
+      const int n_goal = e->es.success_num_conn[env];
+      int success = (nc == n_goal && np > 1) ? 1 : 0;
       int done = success;
       if (e->es.dense) { // FurnitureSawyerEnv._step: reward, _done, info = _compute_reward(a); done = done or _done (furniture_sawyer.py:66-84)
         FeSliceWorld world = {w};
@@ -709,7 +777,7 @@ FE_HD void fe_env_finish(FeEnv* e, const float* a, int act_dim, float connect, i
         for (int k = 0; k < act_dim; ++k) ad[k] = (double)a[k];
         int dd = 0;
         FeDenseState* ds = e->es.dstate + env;
-        fe_dense_step(world, e->es.dense, &sc->dense, thr, np - 1, ds, ad, act_dim, connected_now, &dr, &dd, di);
+        fe_dense_step(world, e->es.dense, &sc->dense, thr, n_goal, ds, ad, act_dim, connected_now, &dr, &dd, di);
         reward = (float)dr;
         success = ds->success;
         done = done || dd;

@@ -262,7 +262,7 @@ class Engine:
         return d.value, e.value
 
     _INT = {"order", "geom_contype", "geom_conaffinity", "eq_active", "touch", "flags", "ncon", "niter", "stats", "con_geom", "con_state", "group", "site_connected",
-            "num_connected", "prev_num_connected", "touched", "picked", "episode_length", "done", "mt_pos"}
+            "num_connected", "prev_num_connected", "touched", "picked", "episode_length", "done", "mt_pos", "preassembled", "num_connects"}
 
     def get(self, name):
         dim, eb = self.field_info(name)
@@ -323,8 +323,30 @@ class Engine:
         self._chk(self.L.fe_set_max_episode_steps(self.h, int(n)))
         self.cfg.max_episode_steps = int(n)
 
+    def set_subtask(self, subtask, num_connects=None):
+        """FurnitureEnv.set_subtask (furniture.py:204-207), per env: `subtask` recipe steps are connected by the env's next reset (an
+        auto-reset included) and the episode then succeeds after `num_connects` more connections (None: when every part is connected).
+        Each is a scalar or an (N,) array; num_connects < 0 in an array stands for None."""
+        k = np.broadcast_to(np.asarray(subtask, dtype=np.int64), (self.N,))
+        nc = np.broadcast_to(np.asarray(-1 if num_connects is None else num_connects, dtype=np.int64), (self.N,))
+        nsub = int(self.scene.dense.nsub)
+        if k.any() and nsub == 0:
+            raise NotImplementedError("preassembled starts follow the furniture's assembly recipe, and this scene packs none (a furniture without "
+                                      "recipes/<name>.yaml, or a two-arm agent)")
+        last = nsub - 1 if (self.dense is not None and nsub > 0) else nsub  # the dense reward needs a subtask left to work on
+        if k.min() < 0 or k.max() > last:
+            raise ValueError("subtask must lie in [0, %d] for this env, got %s" % (last, np.unique(k).tolist()))
+        self.set("preassembled", k[:, None])
+        self.set("num_connects", np.maximum(nc, -1)[:, None])
+
+    def num_subtask(self):
+        """FurnitureEnv.num_subtask (furniture.py:209-213) per env: num_connects where it is set, else the number of parts - 1"""
+        nc = self.get("num_connects")[:, 0]
+        return np.where(nc >= 0, nc, self.scene.npart - 1)
+
     def dense_eval(self, dc, recipe, thr, n_goal, first, count, site_pos, site_mat, part_pos, touch, reset, connected, ac):
-        """test hook fe_dense_eval: the device reward machine on explicit poses, episodes [first[e], first[e] + count[e])"""
+        """test hook fe_dense_eval: the device reward machine on explicit poses, episodes [first[e], first[e] + count[e]); a record with
+        reset = 1 + k starts its episode at subtask k"""
         R, nsite = site_pos.shape[:2]
         npart, act_dim = part_pos.shape[1], ac.shape[1]
         f = lambda a, dt: np.ascontiguousarray(a, dtype=dt)

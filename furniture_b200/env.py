@@ -36,10 +36,21 @@ FURNITURE_NAMES = (
     "three_blocks three_blocks_peg toy_table toy_table_flip tvunit_0406 tvunit_lack_0829 tvunit_lack_0830").split()
 
 
+def prefix_length(preassembled):
+    """`preassembled` of config/furniture.py:158 -> how many recipe steps it names.  The accelerated path starts an episode after the first k
+    steps of the recipe, which is what set_subtask produces (furniture.py:204-207) and what the dense reward assumes
+    (furniture_sawyer_dense.py:128-139): any other list is refused."""
+    p = [int(x) for x in (preassembled if preassembled is not None else ())]
+    if p != list(range(len(p))):
+        raise ValueError("preassembled must be a prefix [0, 1, ..., k-1] of the assembly recipe, got %r" % (list(preassembled),))
+    return len(p)
+
+
 def split_config(config):
     """Reference-style config (argparse Namespace or dict, config/furniture.py) -> (furniture name, FeConfig overrides, ignored keys).
     `furniture_name` wins over `furniture_id` as in furniture.py:157-161; keys the accelerated path has no use for (port, background,
-    camera and rendering options ...) are returned so that callers can report them instead of failing on them."""
+    camera and rendering options ...) are returned so that callers can report them instead of failing on them.  `preassembled` (checked to be
+    a recipe prefix) and `num_connects` travel with the overrides when they are set: they are keywords of the env constructors."""
     from .engine import FeConfig
 
     cfg = dict(vars(config)) if hasattr(config, "__dict__") and not isinstance(config, dict) else dict(config or {})
@@ -54,7 +65,11 @@ def split_config(config):
     fields = {f[0] for f in FeConfig._fields_} - {"struct_bytes"}
     renamed = {"furn_xyz_rand": "furn_xyz_rand", "furn_rot_rand": "furn_rot_rand", "agent_xyz_rand": "agent_xyz_rand", "alignment_pos_dist": "alignment_pos_dist"}
     over = {renamed.get(k, k): v for k, v in cfg.items() if renamed.get(k, k) in fields and v is not None}
-    ignored = sorted(k for k in cfg if k not in over and k not in ("furniture_name", "furniture_id", "control_type"))
+    ignored = sorted(k for k in cfg if k not in over and k not in ("furniture_name", "furniture_id", "control_type", "preassembled", "num_connects"))
+    if prefix_length(cfg.get("preassembled")):
+        over["preassembled"] = list(cfg["preassembled"])
+    if cfg.get("num_connects") is not None:
+        over["num_connects"] = int(cfg["num_connects"])
     return name or "table_lack_0825", over, ignored
 
 
@@ -86,7 +101,7 @@ def split_dense_config(config):
 
 class BatchedFurnitureEnv:
     def __init__(self, agent="Sawyer", furniture_name="table_lack_0825", num_envs=1, device=0, dense=None, control_type="impedance", ik=None,
-                 **cfg_overrides):
+                 preassembled=None, num_connects=None, **cfg_overrides):
         """`dense`: None for the sparse reward of FurnitureEnv; a dict of coefficient overrides (possibly empty) for the phase-based
         reward of FurnitureSawyerDenseRewardEnv, computed inside the step kernel (furniture_b200/dense.py).
         `control_type`: "impedance" (joint velocities, dof 9), "ik" (move 3, rotate 3, gripper, connect: dof 8) or "ik_quaternion" (the
@@ -94,7 +109,9 @@ class BatchedFurnitureEnv:
         step kernel (furniture_b200/ik.py); or one of the NEW_CONTROLLERS ("position", "position_orientation", "joint_impedance",
         "joint_torque", "joint_velocity": the command of the controller, gripper, connect), which switch the scene to the torque-actuated
         robot and evaluate the controller before every mj_step inside the step kernel (furniture_b200/controllers.py); `ik`: overrides of ik.IK_DEFAULTS
-        (move_speed, rotate_speed, action_repeat ...)."""
+        (move_speed, rotate_speed, action_repeat ...).
+        `preassembled`, `num_connects`: config/furniture.py:81, :158 -- the recipe prefix [0, ..., k-1] every env starts its episodes
+        from and the connections that end one; set_subtask changes them per env later."""
         import torch
 
         if not torch.cuda.is_available():
@@ -155,6 +172,18 @@ class BatchedFurnitureEnv:
         self._done = torch.empty(num_envs, dtype=torch.uint8, device=self.device)
         self._info = torch.empty((num_envs, INFO_DIM), dtype=torch.int32, device=self.device)
         self._act = torch.empty((num_envs, self.act_dim), dtype=torch.float32, device=self.device)
+        if prefix_length(preassembled) or num_connects is not None:
+            self.set_subtask(prefix_length(preassembled), num_connects)
+
+    def set_subtask(self, subtask, num_connects=None):
+        """FurnitureEnv.set_subtask (furniture.py:204-207) with a scalar or an (N,) array each, so that the envs of one batch can train different
+        legs of the assembly: env i's next reset (an auto-reset included) connects the first subtask[i] steps of the recipe inside the reset
+        kernel, and its episodes then succeed after num_connects[i] more connections (None: once every part is connected)."""
+        self.engine.set_subtask(subtask, num_connects)
+
+    def num_subtask(self):
+        """FurnitureEnv.num_subtask (furniture.py:209-213) per env, an (N,) array"""
+        return self.engine.num_subtask()
 
     # spaces, in the reference's terms (furniture.py:215-252, :293-310)
     @property

@@ -33,7 +33,7 @@ class FurnitureGymB200:
         """`id`, `name` and the remaining keywords are what gym passes from the registration (env/__init__.py:19-114: id, name,
         furniture_name / furniture_id, background, port ...); options of the renderer are ignored, see env.split_config"""
         from .dense import dense_config
-        from .env import DENSE_IDS, NEW_CONTROLLERS, control_options, split_config, split_dense_config
+        from .env import DENSE_IDS, NEW_CONTROLLERS, control_options, prefix_length, split_config, split_dense_config
 
         if name not in AGENTS:
             raise ValueError("unknown env %s (this build accelerates %s)" % (name, sorted(AGENTS)))
@@ -45,6 +45,7 @@ class FurnitureGymB200:
             self.dense_cfg = dense_config(**dense)
         else:
             furniture_name, over, self.ignored_config = split_config(config)
+        preassembled, num_connects = prefix_length(over.pop("preassembled", None)), over.pop("num_connects", None)
         ctl = control_options(config)
         self.control_type, self.ik_cfg, self.ctl_cfg = ctl["control_type"], None, None
         agent = AGENTS[name]
@@ -79,6 +80,8 @@ class FurnitureGymB200:
         self._pending_ob = None  # observation of an episode the device has already started
         self._episode_reward = 0.0
         self._episode_time = time.time()
+        if preassembled or num_connects is not None:
+            self.set_subtask(preassembled, num_connects)
 
     # ---- spaces (furniture.py:215-252, :293-310): plain shape / bound records, gym.spaces objects when gym is installed
     @property
@@ -150,6 +153,14 @@ class FurnitureGymB200:
     def set_max_episode_steps(self, max_episode_steps):
         self._max_episode_steps = int(max_episode_steps)
         self.engine.set_max_episode_steps(self._max_episode_steps)
+
+    def set_subtask(self, subtask, num_connects=None):
+        """furniture.py:204-207: from the next reset on, episodes start with the first `subtask` recipe steps connected"""
+        self.engine.set_subtask(int(subtask), num_connects)
+        self._pending_ob = None  # an episode the device started on its own still has the old subtask: the next reset() resets again
+
+    def num_subtask(self):
+        return int(self.engine.num_subtask()[0])
 
     def get_env_state(self):
         q, v = self.engine.get_state()

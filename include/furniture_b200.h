@@ -95,7 +95,10 @@ int fe_sim_step(fe_handle* h, int nsub, void* stream);
    qacc_warmstart gravcomp eq_data eq_active geom_contype geom_conaffinity mt_state (624 x uint32) mt_pos (read/write); qfrc_bias link_xpos link_xquat
    link_xmat link_vel touch ncon niter + the debug fields of the last fe_sim_forward (read only); flags (int32, the FE_FLAG_* bits below;
    read/write); stats (int32, one per FE_STAT_* column below; read only); order (int32, one per env: the env ids by the predicted work of their
-   next env step, heaviest first, the order in which the step packs envs into blocks) */
+   next env step, heaviest first, the order in which the step packs envs into blocks); preassembled num_connects (int32, one per env,
+   read/write: FurnitureEnv.set_subtask, furniture.py:204-207.  An env's next reset, an auto-reset included, connects the first `preassembled`
+   steps of the scene's assembly recipe before it places the robot, and the episode then succeeds at num_connects + preassembled connections,
+   or with every part connected when num_connects is -1) */
 int fe_get_field(fe_handle* h, const char* name, void* dst_host, size_t bytes);
 int fe_set_field(fe_handle* h, const char* name, const void* src_host, size_t bytes);
 int fe_field_dim(fe_handle* h, const char* name, int* dim, int* elem_bytes);
@@ -175,7 +178,8 @@ int fe_is_aligned(fe_handle* h, int n, const double* p1, const double* m1, const
                   const int32_t* nangles, const double* thr /* (n,4) */, uint8_t* aligned_host, double* target_quat_host /* (n,4) wxyz, NaN if unset */);
 
 /* ---- test hook: the device reward machine on explicit poses.  Records [first[e], first[e] + count[e]) form episode e and are walked in
- * order by one thread; a record with reset != 0 starts the episode on the world it shows.  Per record: site_pos (nsite,3), site_mat
+ * order by one thread; a record with reset != 0 starts the episode on the world it shows, at subtask reset - 1
+ * (reset = 1 + the number of preassembled recipe steps).  Per record: site_pos (nsite,3), site_mat
  * (nsite,9 row-major), part_pos (npart,3), touch (npart: both fingers on the part), connected, ac (act_dim).  The ids inside the recipe
  * blob index these arrays.  Outputs per record: reward, done (bit 0 done, bit 1 success), info (fe_dense_info_dim() doubles). */
 int fe_dense_eval(fe_handle* h, const fe_dense_config* dc, const void* recipe_blob, size_t recipe_bytes, const double* thr4, int n_goal, int n_episodes,
