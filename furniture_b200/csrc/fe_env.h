@@ -49,6 +49,12 @@ struct FeEnvState {
   int* success_num_conn;                       // [N] _success_num_conn as the env's last reset left it (furniture.py:1477-1481)
   uint32_t* mt;                                // [N][624] MT19937 state of the env's numpy RandomState(seed + env)
   int* mt_pos;                                 // [N] position in the state (624 = regenerate before the next draw)
+  // recorded starts, _init_qpos (furniture.py:121-130, :315-316, :1433-1434): a bank shared by the envs, and per env the entry its resets start from
+  const float *init_qpos, *init_qvel;          // [n_init][nq], [n_init][nv] (fe_set_init_states)
+  int n_init;
+  int *init_state, *init_pick;                 // [N] bank index of the env's _init_qpos, -1 = None; leading entries its resets pick from, 0 = no load_init_states
+  uint32_t* init_mt;                           // [N][624] MT19937 of the pick, numpy RandomState(seed + 2**20 + env); laid out like mt
+  int* init_mt_pos;                            // [N]
   int *robot_contype, *robot_conaff;           // [N][ngeom] saved robot masks during reset
   float* episode_reward;
   // dense (phase-based) reward, fe_dense.h: NULL = the sparse reward of FurnitureEnv._compute_reward
@@ -235,6 +241,16 @@ FE_HD double fe_mt_double(uint32_t* mt, int* pos) {
 }
 // RandomState.uniform(low, high): low + (high - low) * random_sample()
 FE_HD double fe_mt_uniform(uint32_t* mt, int* pos, double lo, double hi) { return ndadd(lo, ndmul(ndsub(hi, lo), fe_mt_double(mt, pos))); }
+// RandomState.randint(0, n), which RandomState.choice(n items) draws: no draw for n = 1, else masked rejection on 32-bit draws
+FE_HD int fe_mt_randint(uint32_t* mt, int* pos, int n) {
+  const uint32_t rng = (uint32_t)(n - 1);
+  if (rng == 0) return 0;
+  uint32_t mask = rng;
+  mask |= mask >> 1; mask |= mask >> 2; mask |= mask >> 4; mask |= mask >> 8; mask |= mask >> 16;
+  uint32_t v;
+  do v = fe_mt_u32(mt, pos) & mask; while (v > rng);
+  return (int)v;
+}
 
 // ---------------------------------------------------------------- env context of one warp
 // Scratch of the connect path, the re-pin and the auto-reset: values lane 0 hands to the other lanes and to later parts of the step
@@ -372,8 +388,10 @@ FE_FN void fe_try_connect_scan(FeEnv* e, int part1) {
 }
 
 // _connect(site1, site2, auto_align) (furniture.py:847-924) for arm agents: the pair in si->site1 .. conn2, its target quat in sd->target_quat.
-// `force_align`: align the connectors whatever cfg->auto_align says (the reset's preassembly, furniture.py:1556)
-FE_FN void fe_connect(FeEnv* e, bool force_align) {
+// `align`: FE_ALIGN_CONFIG follows cfg->auto_align (a connection made by the policy); the reset's preassembly passes auto_align=_init_qpos is None
+// (furniture.py:1556): FE_ALIGN_ALWAYS after random placement, FE_ALIGN_NEVER on a recorded start
+enum { FE_ALIGN_CONFIG = 0, FE_ALIGN_ALWAYS = 1, FE_ALIGN_NEVER = 2 };
+FE_FN void fe_connect(FeEnv* e, int align) {
   FeWarp* w = e->w;
   const fe_model* m = w->m;
   const fe_scene* sc = e->sc;
@@ -389,7 +407,7 @@ FE_FN void fe_connect(FeEnv* e, bool force_align) {
         const int gp = fe_find(e->group, p);
         if ((gp == g1 || gp == g2) && w->contype()[g] != 0) { w->contype()[g] = (1 << 30) - 1 - (1 << (g1 + 1)); w->conaff()[g] = 1 << (g1 + 1); }
       }
-      if (e->cfg->auto_align || force_align) { // _align_connectors -> _move_site_to_target (furniture.py:1224-1250)
+      if (align == FE_ALIGN_ALWAYS || (align == FE_ALIGN_CONFIG && e->cfg->auto_align)) { // _align_connectors -> _move_site_to_target (furniture.py:1224-1250)
         double target[7], base[7], sp[3], sq[4];
         fe_site_pose_d(w, s1, sp, nullptr, sq);
         for (int k = 0; k < 3; ++k) target[k] = sp[k];
@@ -551,14 +569,14 @@ FE_FN void fe_env_preassemble_pair(FeEnv* e, int i) {
   LANES_END
 }
 
-// FurnitureEnv._reset (furniture.py:1406-1663) in two calls with the preassembly between them (fe_env_reset_one), so that its connect path does
-// not stack on their frames: up to the furniture at rest, with `pre` recipe steps to preassemble, and from the robot's pose on
-FE_FN void fe_env_reset_furniture(FeEnv* e, int pre) {
+// FurnitureEnv._reset (furniture.py:1406-1663) in non-inlined parts called one after the other by fe_env_reset_one, so that the connect path of
+// the preassembly does not stack on their frames.  This one, shared by both branches of `if self._init_qpos:`: the size-factor draw, sim.reset()
+// and the episode's bookkeeping with the robot's collisions off (:1428-1503), `pre` recipe steps to preassemble
+FE_FN void fe_env_reset_clear(FeEnv* e, int pre) {
   FeWarp* w = e->w;
   const fe_model* m = w->m;
-  const fe_scene* sc = e->sc;
   const fe_config* cfg = e->cfg;
-  const int nr = m->nr, nrl = m->nrlink, np = m->npart, ng = m->ngeom;
+  const int nr = m->nr, np = m->npart, ng = m->ngeom;
   int* rct = e->es.robot_contype + (size_t)e->env * ng;
   int* rca = e->es.robot_conaff + (size_t)e->env * ng;
   LANES_BEGIN
@@ -581,13 +599,25 @@ FE_FN void fe_env_reset_furniture(FeEnv* e, int pre) {
       e->es.success_num_conn[e->env] = ask >= 0 ? ask + pre : np - 1; // furniture.py:1477-1481
       e->si->aligned = 0;                                             // _connected = False (:1468)
       w->u()[FE_U_FLAGS] = 0;
+      if (cfg->furn_size_rand != 0.f) { // _reset draws a size factor first (furniture.py:1428-1431; it only edits the XML tree)
+        int pos = e->es.mt_pos[e->env];
+        (void)fe_mt_double(e->es.mt + (size_t)e->env * FE_MT_N, &pos);
+        e->es.mt_pos[e->env] = pos;
+      }
     }
   LANES_END
+}
+// _place_objects and the first settle loop (:1519-1540)
+FE_FN void fe_env_reset_place(FeEnv* e) {
+  FeWarp* w = e->w;
+  const fe_model* m = w->m;
+  const fe_scene* sc = e->sc;
+  const fe_config* cfg = e->cfg;
+  const int nrl = m->nrlink, np = m->npart;
   LANES_BEGIN
     if (lane == 0) { // UniformRandomSampler.sample (placement_sampler.py:137-190): xy noise, z + 0.01, +furn_rot_rand deg about x
       uint32_t* mt = e->es.mt + (size_t)e->env * FE_MT_N;
       int pos = e->es.mt_pos[e->env];
-      if (cfg->furn_size_rand != 0.f) (void)fe_mt_double(mt, &pos); // _reset draws a size factor first (furniture.py:1428-1431; it only edits the XML tree)
       const double half = 0.5 * (double)cfg->furn_rot_rand * 3.14159265358979323846 / 180.0;
       const double qx[4] = {cos(half), sin(half), 0.0, 0.0};
       const double r_xy = (double)cfg->furn_xyz_rand, r_rot = (double)cfg->furn_rot_rand;
@@ -617,12 +647,13 @@ FE_FN void fe_env_reset_furniture(FeEnv* e, int pre) {
   LANES_END
   fe_env_stabilise(e);
 }
-FE_FN void fe_env_reset_robot(FeEnv* e, int pre) {
+// gravity compensation and 101 robot poses, the second one with the robot's collisions back on (:1569-1612)
+FE_FN void fe_env_reset_robot(FeEnv* e) {
   FeWarp* w = e->w;
   const fe_model* m = w->m;
   const fe_scene* sc = e->sc;
   const fe_config* cfg = e->cfg;
-  const int nr = m->nr, np = m->npart, ng = m->ngeom;
+  const int ng = m->ngeom;
   const int* rct = e->es.robot_contype + (size_t)e->env * ng;
   const int* rca = e->es.robot_conaff + (size_t)e->env * ng;
   // gravity compensation, robot pose, one step with robot collisions still off (furniture.py:1569-1584)
@@ -644,7 +675,14 @@ FE_FN void fe_env_reset_robot(FeEnv* e, int pre) {
     LANES_END
     fe_fwd_step(e);
   }
-  // sync (furniture.py:1621-1628), gravity compensation from that forward pass, 100 settle steps (:1639-1641)
+}
+// shared by both branches again: the sync block (furniture.py:1621-1628), gravity compensation from that forward pass, 100 settle steps
+// (:1639-1641), the episode's first observation
+FE_FN void fe_env_reset_sync(FeEnv* e, int pre) {
+  FeWarp* w = e->w;
+  const fe_model* m = w->m;
+  const fe_scene* sc = e->sc;
+  const int nr = m->nr, np = m->npart;
   LANES_BEGIN
     for (int i = lane; i < m->nu; i += 32) w->ctrl()[i] = 0.f;
     for (int i = lane; i < nr; i += 32) w->qfrc_applied()[i] = 0.f;
@@ -669,15 +707,69 @@ FE_FN void fe_env_reset_robot(FeEnv* e, int pre) {
   LANES_END
   fe_write_obs(e);
 }
+// set_env_state(_init_qpos) (furniture.py:1794-1798) from bank entry s: _stop_objects(gravity=0), qpos and qvel, ctrl = 0.  `robot`: the first call
+// of the reset, which switches the robot's collisions back on (:1505-1517)
+FE_FN void fe_env_set_init_state(FeEnv* e, int s, bool robot) {
+  FeWarp* w = e->w;
+  const fe_model* m = w->m;
+  const int ng = m->ngeom;
+  const int* rct = e->es.robot_contype + (size_t)e->env * ng;
+  const int* rca = e->es.robot_conaff + (size_t)e->env * ng;
+  const float* q = e->es.init_qpos + (size_t)s * m->nq;
+  const float* v = e->es.init_qvel + (size_t)s * m->nv;
+  LANES_BEGIN
+    for (int p = lane; p < m->npart; p += 32) w->gravcomp()[p] = 0.f;
+    for (int i = lane; i < m->nq; i += 32) w->qpos()[i] = q[i];
+    for (int i = lane; i < m->nv; i += 32) w->qvel()[i] = v[i];
+    for (int i = lane; i < m->nu; i += 32) w->ctrl()[i] = 0.f;
+    if (robot) for (int g = lane; g < ng; g += 32) if (m->geom_tag[g] & FE_TAG_ROBOT) { w->contype()[g] = rct[g]; w->conaff()[g] = rca[g]; }
+  LANES_END
+}
+// the pick before every reset (furniture.py:1433-1434): `if np.random.rand() > 0.2: set_init_qpos(np.random.choice(states))` over the first
+// init_pick bank entries, drawn from the env's init_mt; a failed draw keeps the env's start.  Returns the start, -1 = None (random placement);
+// an index past the bank counts as None
+FE_FN int fe_env_pick_start(FeEnv* e) {
+  const int env = e->env, n_init = e->es.n_init;
+  LANES_BEGIN
+    if (lane == 0) {
+      const int n = e->es.init_pick[env] < n_init ? e->es.init_pick[env] : n_init;
+      if (n > 0) {
+        uint32_t* mt = e->es.init_mt + (size_t)env * FE_MT_N;
+        int pos = e->es.init_mt_pos[env];
+        if (fe_mt_double(mt, &pos) > 0.2) e->es.init_state[env] = fe_mt_randint(mt, &pos, n);
+        e->es.init_mt_pos[env] = pos;
+      }
+    }
+  LANES_END
+  const int s = e->es.init_state[env];
+  return s < n_init ? s : -1;
+}
 // the warp slice is (re)initialised here, caller stores it
 FE_FN void fe_env_reset_one(FeEnv* e) {
   const fe_scene* sc = e->sc;
   const int want = e->es.preassembled[e->env], cap = sc->dense.nsub - (e->es.dense && sc->dense.nsub > 0 ? 1 : 0); // a recipe prefix; the dense reward needs a subtask left
   const int pre = want < 0 ? 0 : (want > cap ? cap : want);
-  fe_env_reset_furniture(e, pre);
-  for (int i = 0; i < pre; ++i) { fe_env_preassemble_pair(e, i); fe_connect(e, true); } // :1542-1558, robot collisions still off
-  if (pre > 0) fe_env_stabilise(e);                                                      // :1560-1566
-  fe_env_reset_robot(e, pre);
+  const int s = fe_env_pick_start(e);
+  fe_env_reset_clear(e, pre);
+  if (s < 0) {
+    fe_env_reset_place(e);
+    for (int i = 0; i < pre; ++i) { fe_env_preassemble_pair(e, i); fe_connect(e, FE_ALIGN_ALWAYS); } // :1542-1558, robot collisions still off
+    if (pre > 0) fe_env_stabilise(e);                                                                // :1560-1566
+    fe_env_reset_robot(e);
+  } else { // `if self._init_qpos:` (:1505-1518): no placement, no settle loop, no random draw; the parts start unwelded
+    fe_env_set_init_state(e, s, true);
+    fe_forward(e->w);
+    for (int i = 0; i < pre; ++i) { fe_env_preassemble_pair(e, i); fe_connect(e, FE_ALIGN_NEVER); } // :1542-1558, robot collisions on
+    // The settle loop after the preassembly (:1560-1566) and the forward pass of :1568 are skipped: the second set_env_state (:1617) and the
+    // sync block (:1621-1627) overwrite all they produce (qpos, qvel, xfrc, qfrc, warmstart, time); the welds' eq_data is set before them.
+    fe_env_set_init_state(e, s, false);
+  }
+  fe_env_reset_sync(e, pre);
+}
+// the reset of _do_simulation's except branch (furniture.py:2889-2897), which clears the env's start first: set_init_qpos(None)
+FE_HD void fe_env_reset_unstable(FeEnv* e) {
+  LANES_BEGIN if (lane == 0) e->es.init_state[e->env] = -1; LANES_END
+  fe_env_reset_one(e);
 }
 
 // the per-step flags: no connection found, no re-pin pending, no auto-reset due, no simulation failure yet (lane 0)
@@ -717,7 +809,7 @@ FE_HD void fe_env_finish(FeEnv* e, const float* a, int act_dim, float connect, i
   const int np = m->npart, env = e->env;
   FE_SYNC;
   if (reset_now) {
-    fe_env_reset_one(e);
+    fe_env_reset_unstable(e);
   } else {
     if (connect > 0.f) { // furniture.py:1290-1322: per arm, the first part both of its fingers touch; stop at the first connection
       for (int arm = 0; arm < sc->narms; ++arm) {
@@ -726,7 +818,7 @@ FE_HD void fe_env_finish(FeEnv* e, const float* a, int act_dim, float connect, i
         for (int p = 0; p < np; ++p) if ((w->touch()[p] & both) == both) { part = p; break; }
         if (part >= 0) {
           fe_try_connect_scan(e, part);
-          if (e->si->aligned) { fe_connect(e, false); break; }
+          if (e->si->aligned) { fe_connect(e, FE_ALIGN_CONFIG); break; }
         }
       }
     }
@@ -742,7 +834,9 @@ FE_HD void fe_env_finish(FeEnv* e, const float* a, int act_dim, float connect, i
         }
       LANES_END
       fe_fwd_step(e);
-      if (w->u()[FE_U_FLAGS] & FE_FLAG_DIVERGED) { fail = 1; fe_env_reset_one(e); }
+      // the re-pin step diverged: the device's stand-in for the reference, whose re-pin step has no except branch and would raise.  The
+      // episode ends as an unstable one, and the reset clears the env's start as _do_simulation's except branch does.
+      if (w->u()[FE_U_FLAGS] & FE_FLAG_DIVERGED) { fail = 1; fe_env_reset_unstable(e); }
     }
   }
   // reward (furniture.py:482-541), termination (:440-445, :451-480)

@@ -229,7 +229,7 @@ FE_FN void fe_env_ik_step_one(FeEnv* e, FeIkArgs ik, const float* action, float*
     if (w->u()[FE_U_FLAGS] & FE_FLAG_DIVERGED) { // _do_simulation's except branch: reset, then the remaining repeats run on the new episode (furniture.py:2889-2897)
       fail = 1;
       FE_SYNC;
-      if (r + 1 < c->action_repeat) fe_env_reset_one(e); else reset_now = 1;
+      if (r + 1 < c->action_repeat) fe_env_reset_unstable(e); else reset_now = 1;
     }
   }
   fe_env_finish(e, a, act_dim, connect, fail, reset_now, reward_out, done_out, info_out);

@@ -236,6 +236,7 @@ class Engine:
         if controller is not None:  # one of the NEW_CONTROLLERS (furniture_b200/controllers.py: FeCtlConfig) on the torque-actuated robot
             self._chk(L.fe_enable_controller(self.h, C.byref(controller)))
             self.act_dim = int(L.fe_action_dim(self.h))
+        self._bank, self._n_pick = [], 0  # host copy of the bank of recorded starts; its first _n_pick entries are the load_init_states list
         self.dense = dense
         if dense is not None:  # FurnitureSawyerDenseRewardEnv: the phase machine replaces the sparse reward inside fe_env_step
             self._chk(L.fe_enable_dense_reward(self.h, C.byref(dense)))
@@ -262,18 +263,20 @@ class Engine:
         return d.value, e.value
 
     _INT = {"order", "geom_contype", "geom_conaffinity", "eq_active", "touch", "flags", "ncon", "niter", "stats", "con_geom", "con_state", "group", "site_connected",
-            "num_connected", "prev_num_connected", "touched", "picked", "episode_length", "done", "mt_pos", "preassembled", "num_connects"}
+            "num_connected", "prev_num_connected", "touched", "picked", "episode_length", "done", "mt_pos", "preassembled", "num_connects",
+            "init_state", "init_pick", "init_mt_pos"}
+    _U32 = {"mt_state", "init_mt_state"}
 
     def get(self, name):
         dim, eb = self.field_info(name)
-        dt = np.uint8 if eb == 1 else np.uint64 if eb == 8 else (np.uint32 if name == "mt_state" else (np.int32 if name in self._INT else np.float32))
+        dt = np.uint8 if eb == 1 else np.uint64 if eb == 8 else (np.uint32 if name in self._U32 else (np.int32 if name in self._INT else np.float32))
         out = np.empty((self.N, dim), dtype=dt)
         self._chk(self.L.fe_get_field(self.h, name.encode(), out.ctypes.data_as(C.c_void_p), C.c_size_t(out.nbytes)))
         return out
 
     def set(self, name, value):
         dim, eb = self.field_info(name)
-        dt = np.uint8 if eb == 1 else np.uint64 if eb == 8 else (np.uint32 if name == "mt_state" else (np.int32 if name in self._INT else np.float32))
+        dt = np.uint8 if eb == 1 else np.uint64 if eb == 8 else (np.uint32 if name in self._U32 else (np.int32 if name in self._INT else np.float32))
         v = np.ascontiguousarray(np.broadcast_to(np.asarray(value, dtype=dt), (self.N, dim)))
         self._chk(self.L.fe_set_field(self.h, name.encode(), v.ctypes.data_as(C.c_void_p), C.c_size_t(v.nbytes)))
 
@@ -343,6 +346,82 @@ class Engine:
         """FurnitureEnv.num_subtask (furniture.py:209-213) per env: num_connects where it is set, else the number of parts - 1"""
         nc = self.get("num_connects")[:, 0]
         return np.where(nc >= 0, nc, self.scene.npart - 1)
+
+    # ---- recorded starts: _init_qpos, --load_init_states, --load_demo (furniture.py:121-130, :315-316, :1433-1434)
+    def _state_arrays(self, state):
+        """a get_env_state dict -> (qpos, qvel) float32 of this handle's model, or ValueError"""
+        try:
+            q = np.asarray(state["qpos"], dtype=np.float64).ravel()
+            v = np.asarray(state["qvel"], dtype=np.float64).ravel()
+        except (KeyError, TypeError, ValueError) as e:
+            raise ValueError("a state is a dict with numeric 'qpos' and 'qvel' (get_env_state), got %r" % (type(state),)) from e
+        if q.size != self.model.nq or v.size != self.model.nv:
+            raise ValueError("state has qpos / qvel of length %d / %d, this model has nq = %d, nv = %d" % (q.size, v.size, self.model.nq, self.model.nv))
+        if not (np.isfinite(q).all() and np.isfinite(v).all()):
+            raise ValueError("state holds non-finite qpos / qvel")
+        return q.astype(np.float32), v.astype(np.float32)
+
+    def set_init_states(self, states):
+        """fe_set_init_states: the bank of recorded starts every env of the handle indexes with its `init_state` / `init_pick` fields, a list
+        of get_env_state dicts ([] or None frees it).  The fields are left as they are; set_init_qpos and load_init_states manage both."""
+        arrs = [self._state_arrays(st) for st in (states or [])]
+        self._upload_bank(arrs)
+        self._n_pick = min(self._n_pick, len(arrs))
+
+    def _upload_bank(self, arrs):
+        nq, nv = self.model.nq, self.model.nv
+        q = np.ascontiguousarray(np.array([a[0] for a in arrs], np.float32).reshape(len(arrs), nq))
+        v = np.ascontiguousarray(np.array([a[1] for a in arrs], np.float32).reshape(len(arrs), nv))
+        self._chk(self.L.fe_set_init_states(self.h, q.ctypes.data_as(C.c_void_p), v.ctypes.data_as(C.c_void_p), len(arrs)))
+        self._bank = list(arrs)
+
+    def _rebank(self, head, extra):
+        """bank = head (the pick list) + every other entry an env starts from + extra; remaps init_state and returns the index of extra[0]"""
+        cur = self.get("init_state")[:, 0]
+        used = sorted({int(s) for s in cur if s >= 0})
+        keep = [s for s in used if head is not None or s >= self._n_pick]  # a new list keeps every start in use, wherever it sat
+        head_arrs = self._bank[: self._n_pick] if head is None else head
+        remap = {s: s for s in used if s not in keep}
+        remap.update({s: len(head_arrs) + i for i, s in enumerate(keep)})
+        self._upload_bank(list(head_arrs) + [self._bank[s] for s in keep] + list(extra))
+        self.set("init_state", np.array([remap.get(int(s), -1) for s in cur], np.int32)[:, None])
+        return len(head_arrs) + len(keep)
+
+    def set_init_qpos(self, states):
+        """FurnitureEnv.set_init_qpos (furniture.py:315-316) per env: `states` is one get_env_state dict or None for every env, or a list of
+        N such entries.  From its next reset on (an auto-reset included) an env with a state starts from it, and None goes back to random
+        placement; a load_init_states pick may later replace it, an unstable step clears it."""
+        per_env = isinstance(states, (list, tuple))
+        if per_env and len(states) != self.N:
+            raise ValueError("set_init_qpos takes one state or None for all envs, or a list of %d (one per env), got %d" % (self.N, len(states)))
+        entries = list(states) if per_env else [states] * self.N
+        distinct, slot = [], {}
+        for st in entries:  # the same dict given to many envs is one bank entry
+            if st is not None and id(st) not in slot:
+                slot[id(st)] = len(distinct)
+                distinct.append(self._state_arrays(st))
+        self.set("init_state", np.full((self.N, 1), -1, np.int32))
+        first = self._rebank(None, distinct)
+        self.set("init_state", np.array([-1 if st is None else first + slot[id(st)] for st in entries], np.int32)[:, None])
+
+    def load_init_states(self, states, envs=None):
+        """--load_init_states (furniture.py:127-130, :1433-1434): the handle's list of recorded starts, a list of get_env_state dicts.  Before
+        each of its resets an env in `envs` (default: all) keeps its start with probability 0.2 and otherwise picks one from the list
+        uniformly, drawing from its own numpy RandomState(seed + 2**20 + env); the other envs do not pick.  [] or None ends the picking."""
+        arrs = [self._state_arrays(st) for st in (states or [])]
+        idx = np.arange(self.N) if envs is None else np.asarray(envs, dtype=np.int64).ravel()
+        if idx.size and (idx.min() < 0 or idx.max() >= self.N):
+            raise ValueError("envs must index the %d envs of this handle, got %s" % (self.N, idx.tolist()))
+        self._rebank(arrs, [])
+        self._n_pick = len(arrs)
+        pick = np.zeros(self.N, np.int32)
+        pick[idx] = len(arrs)
+        self.set("init_pick", pick[:, None])
+
+    def init_states(self):
+        """the bank of recorded starts as the device holds it: (qpos (S, nq), qvel (S, nv)) float32, and the length of the pick list"""
+        nq, nv = self.model.nq, self.model.nv
+        return (np.array([a[0] for a in self._bank], np.float32).reshape(-1, nq), np.array([a[1] for a in self._bank], np.float32).reshape(-1, nv), self._n_pick)
 
     def dense_eval(self, dc, recipe, thr, n_goal, first, count, site_pos, site_mat, part_pos, touch, reset, connected, ac):
         """test hook fe_dense_eval: the device reward machine on explicit poses, episodes [first[e], first[e] + count[e]); a record with

@@ -11,6 +11,7 @@ collective is one NCCL all_gather of the packed [obs | reward | done] tensor per
 """
 from __future__ import annotations
 
+import os
 from collections import OrderedDict
 
 import numpy as np
@@ -50,7 +51,8 @@ def split_config(config):
     """Reference-style config (argparse Namespace or dict, config/furniture.py) -> (furniture name, FeConfig overrides, ignored keys).
     `furniture_name` wins over `furniture_id` as in furniture.py:157-161; keys the accelerated path has no use for (port, background,
     camera and rendering options ...) are returned so that callers can report them instead of failing on them.  `preassembled` (checked to be
-    a recipe prefix) and `num_connects` travel with the overrides when they are set: they are keywords of the env constructors."""
+    a recipe prefix), `num_connects`, `load_init_states` and `load_demo` travel with the overrides when they are set: they are keywords of the
+    env constructors."""
     from .engine import FeConfig
 
     cfg = dict(vars(config)) if hasattr(config, "__dict__") and not isinstance(config, dict) else dict(config or {})
@@ -65,11 +67,15 @@ def split_config(config):
     fields = {f[0] for f in FeConfig._fields_} - {"struct_bytes"}
     renamed = {"furn_xyz_rand": "furn_xyz_rand", "furn_rot_rand": "furn_rot_rand", "agent_xyz_rand": "agent_xyz_rand", "alignment_pos_dist": "alignment_pos_dist"}
     over = {renamed.get(k, k): v for k, v in cfg.items() if renamed.get(k, k) in fields and v is not None}
-    ignored = sorted(k for k in cfg if k not in over and k not in ("furniture_name", "furniture_id", "control_type", "preassembled", "num_connects"))
+    ignored = sorted(k for k in cfg if k not in over and k not in ("furniture_name", "furniture_id", "control_type", "preassembled", "num_connects",
+                                                                   "load_init_states", "load_demo"))
     if prefix_length(cfg.get("preassembled")):
         over["preassembled"] = list(cfg["preassembled"])
     if cfg.get("num_connects") is not None:
         over["num_connects"] = int(cfg["num_connects"])
+    for k in ("load_init_states", "load_demo"):  # paths of pickles (furniture.py:121-130), read by the env constructors
+        if cfg.get(k):
+            over[k] = cfg[k]
     return name or "table_lack_0825", over, ignored
 
 
@@ -99,9 +105,22 @@ def split_dense_config(config):
     return name, over, dense, [k for k in ignored if k not in DENSE_DEFAULTS]
 
 
+def apply_init_config(env, load_init_states=None, load_demo=None):
+    """the constructor half of furniture.py:121-130 for an env with set_init_qpos / load_init_states: `load_demo` sets every env's start to
+    the first state of that demo, `load_init_states` gives every env the list to pick from (as every VecEnv worker loads the same file).
+    Each is a path, read with demo.load_init_states, or the list of states itself."""
+    from .demo import load_init_states as read
+
+    states = lambda x: read(x) if isinstance(x, (str, bytes, os.PathLike)) else list(x)
+    if load_demo:
+        env.set_init_qpos(states(load_demo)[0])
+    if load_init_states:
+        env.load_init_states(states(load_init_states))
+
+
 class BatchedFurnitureEnv:
     def __init__(self, agent="Sawyer", furniture_name="table_lack_0825", num_envs=1, device=0, dense=None, control_type="impedance", ik=None,
-                 preassembled=None, num_connects=None, **cfg_overrides):
+                 preassembled=None, num_connects=None, load_init_states=None, load_demo=None, **cfg_overrides):
         """`dense`: None for the sparse reward of FurnitureEnv; a dict of coefficient overrides (possibly empty) for the phase-based
         reward of FurnitureSawyerDenseRewardEnv, computed inside the step kernel (furniture_b200/dense.py).
         `control_type`: "impedance" (joint velocities, dof 9), "ik" (move 3, rotate 3, gripper, connect: dof 8) or "ik_quaternion" (the
@@ -111,7 +130,9 @@ class BatchedFurnitureEnv:
         robot and evaluate the controller before every mj_step inside the step kernel (furniture_b200/controllers.py); `ik`: overrides of ik.IK_DEFAULTS
         (move_speed, rotate_speed, action_repeat ...).
         `preassembled`, `num_connects`: config/furniture.py:81, :158 -- the recipe prefix [0, ..., k-1] every env starts its episodes
-        from and the connections that end one; set_subtask changes them per env later."""
+        from and the connections that end one; set_subtask changes them per env later.
+        `load_init_states`, `load_demo`: config/furniture.py's paths (furniture.py:121-130), or the states themselves: every env picks its
+        starts from the list of `load_init_states` (see load_init_states), and every env starts from the first state of the demo `load_demo`."""
         import torch
 
         if not torch.cuda.is_available():
@@ -174,6 +195,23 @@ class BatchedFurnitureEnv:
         self._act = torch.empty((num_envs, self.act_dim), dtype=torch.float32, device=self.device)
         if prefix_length(preassembled) or num_connects is not None:
             self.set_subtask(prefix_length(preassembled), num_connects)
+        apply_init_config(self, load_init_states, load_demo)
+
+    def set_init_qpos(self, states):
+        """FurnitureEnv.set_init_qpos (furniture.py:315-316), per env: one get_env_state dict or None for all envs, or a list of num_envs of
+        them.  An env with a state starts its episodes from it, from its next reset on (auto-resets included), until an unstable step or a
+        pick of load_init_states replaces it; None goes back to random placement."""
+        self.engine.set_init_qpos(states)
+
+    def load_init_states(self, states, envs=None):
+        """--load_init_states (furniture.py:127-130, :1433-1434): before each reset, an env in `envs` (default: all) keeps its start with
+        probability 0.2 and otherwise starts from a state drawn uniformly from `states` (a list of get_env_state dicts, e.g.
+        demo.load_init_states(path)).  The draw runs inside the reset kernel on the env's own generator."""
+        self.engine.load_init_states(states, envs)
+
+    def set_init_states(self, states):
+        """the raw bank of recorded starts that the per-env fields init_state / init_pick index (Engine.set_init_states)"""
+        self.engine.set_init_states(states)
 
     def set_subtask(self, subtask, num_connects=None):
         """FurnitureEnv.set_subtask (furniture.py:204-207) with a scalar or an (N,) array each, so that the envs of one batch can train different

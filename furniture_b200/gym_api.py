@@ -33,7 +33,7 @@ class FurnitureGymB200:
         """`id`, `name` and the remaining keywords are what gym passes from the registration (env/__init__.py:19-114: id, name,
         furniture_name / furniture_id, background, port ...); options of the renderer are ignored, see env.split_config"""
         from .dense import dense_config
-        from .env import DENSE_IDS, NEW_CONTROLLERS, control_options, prefix_length, split_config, split_dense_config
+        from .env import DENSE_IDS, NEW_CONTROLLERS, apply_init_config, control_options, prefix_length, split_config, split_dense_config
 
         if name not in AGENTS:
             raise ValueError("unknown env %s (this build accelerates %s)" % (name, sorted(AGENTS)))
@@ -46,6 +46,7 @@ class FurnitureGymB200:
         else:
             furniture_name, over, self.ignored_config = split_config(config)
         preassembled, num_connects = prefix_length(over.pop("preassembled", None)), over.pop("num_connects", None)
+        load_init_states, load_demo = over.pop("load_init_states", None), over.pop("load_demo", None)
         ctl = control_options(config)
         self.control_type, self.ik_cfg, self.ctl_cfg = ctl["control_type"], None, None
         agent = AGENTS[name]
@@ -82,6 +83,7 @@ class FurnitureGymB200:
         self._episode_time = time.time()
         if preassembled or num_connects is not None:
             self.set_subtask(preassembled, num_connects)
+        apply_init_config(self, load_init_states, load_demo)
 
     # ---- spaces (furniture.py:215-252, :293-310): plain shape / bound records, gym.spaces objects when gym is installed
     @property
@@ -161,6 +163,17 @@ class FurnitureGymB200:
 
     def num_subtask(self):
         return int(self.engine.num_subtask()[0])
+
+    def set_init_qpos(self, init_qpos):
+        """furniture.py:315-316 (FurnitureGym, furniture_gym.py:43): from the next reset on, episodes start from this get_env_state dict, or
+        from random placement for None"""
+        self.engine.set_init_qpos(init_qpos)
+        self._pending_ob = None  # an episode the device started on its own still has the old start: the next reset() resets again
+
+    def load_init_states(self, states):
+        """--load_init_states (furniture.py:127-130): before each reset, keep the start with probability 0.2, else pick one from `states`"""
+        self.engine.load_init_states(states)
+        self._pending_ob = None
 
     def get_env_state(self):
         q, v = self.engine.get_state()

@@ -10,6 +10,7 @@
  *   fe_set_field/fe_get_field <- sim.data.* / sim.model.* views     furniture.py:1622-1627, :2784-2800, :875-878, :2772-2775
  *   fe_get_state/fe_set_state <- get_env_state / set_env_state      furniture/env/furniture.py:1781-1803, :3095-3105
  *   fe_env_reset     <- FurnitureEnv.reset() -> _reset()             furniture/env/furniture.py:318-334, :1406-1663
+ *   fe_set_init_states <- the states of --load_init_states / --load_demo / set_init_qpos   furniture.py:121-130, :315-316
  *   fe_env_step      <- FurnitureEnv.step() (incl. _step_continuous, _try_connect/_is_aligned/_connect, _get_obs,
  *                       _compute_reward, _after_step; VecEnv auto-reset) furniture.py:364-385, :405-449, :1260-1330,
  *                       :926-1153, :847-924, furniture_sawyer.py:66-155, util/subproc_vec_env.py:16-20
@@ -98,12 +99,22 @@ int fe_sim_step(fe_handle* h, int nsub, void* stream);
    next env step, heaviest first, the order in which the step packs envs into blocks); preassembled num_connects (int32, one per env,
    read/write: FurnitureEnv.set_subtask, furniture.py:204-207.  An env's next reset, an auto-reset included, connects the first `preassembled`
    steps of the scene's assembly recipe before it places the robot, and the episode then succeeds at num_connects + preassembled connections,
-   or with every part connected when num_connects is -1) */
+   or with every part connected when num_connects is -1); init_state init_pick init_mt_state (624 x uint32) init_mt_pos (int32, one per env,
+   read/write: the env's recorded start, see fe_set_init_states) */
 int fe_get_field(fe_handle* h, const char* name, void* dst_host, size_t bytes);
 int fe_set_field(fe_handle* h, const char* name, const void* src_host, size_t bytes);
 int fe_field_dim(fe_handle* h, const char* name, int* dim, int* elem_bytes);
 int fe_get_state(fe_handle* h, float* qpos_host, float* qvel_host);
 int fe_set_state(fe_handle* h, const float* qpos_host, const float* qvel_host);
+/* Recorded starts, FurnitureEnv._init_qpos (furniture.py:121-130, :315-316, :1433-1434, :1505-1518, :1617): a bank of n_states
+   get_env_state records, qpos (n_states, nq) and qvel (n_states, nv) from host memory, shared by the envs of the handle; n_states = 0 frees it.
+   Non-finite values are refused.  Per env, field init_state is the bank index its resets start from (-1 = None: random placement).  Such a
+   reset, an auto-reset included, plants the state instead of placing the parts and posing the robot: the parts start unwelded, the first
+   `preassembled` recipe steps are connected without aligning the connectors, the state is planted again and 100 mj_steps settle it.
+   Field init_pick = n > 0 is --load_init_states over the first n bank entries: before every reset, if rand() > 0.2, init_state = choice(n),
+   drawn from the env's own numpy RandomState(seed + 2**20 + env) (init_mt_state / init_mt_pos), else the env keeps its start.  A reset
+   after an unstable step sets init_state to -1 first (furniture.py:2895).  An index past the bank counts as None. */
+int fe_set_init_states(fe_handle* h, const float* qpos_host, const float* qvel_host, int n_states);
 
 /* Bits of `flags`.  A call ORs in the bits an env raised during it (the step kernels clear an env's bits when they set its controls
    and when they reset it); the field keeps them until the caller writes it. */

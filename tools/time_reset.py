@@ -1,9 +1,11 @@
 """Time one fe_env_reset of a batch with nothing preassembled and with k recipe steps preassembled (CUDA events, one GPU).
 
-  python tools/time_reset.py [--envs 4096] [--k 3] [--repeats 5] [--reward sparse|dense]
+  python tools/time_reset.py [--envs 4096] [--k 3] [--repeats 5] [--reward sparse|dense] [--init-state]
 
 Prints one JSON line: milliseconds per reset launch for k = 0 and for k (median and spread over the repeats, after one warm-up
-reset of each), with the card's name and power limit, which belong beside the numbers.
+reset of each), with the card's name, power limit and the SM clock read right after the timed launches, which belong beside the numbers.  --init-state adds the same two
+times for a batch whose envs all start from a recorded state (set_init_qpos): the state env 0 reached by the random reset with the
+same k, so that the recipe's connectors already touch where the preassembly connects them.
 """
 import argparse
 import json
@@ -20,6 +22,7 @@ def main():
     ap.add_argument("--k", type=int, default=3)
     ap.add_argument("--repeats", type=int, default=5)
     ap.add_argument("--reward", default="sparse", choices=["sparse", "dense"])
+    ap.add_argument("--init-state", action="store_true")
     args = ap.parse_args()
     import torch
 
@@ -29,12 +32,7 @@ def main():
 
     env = BatchedFurnitureEnv("Sawyer", "table_lack_0825", args.envs, dense={} if args.reward == "dense" else None)
     out = {"envs": args.envs, "reward": args.reward, "gpu": torch.cuda.get_device_name(0)}
-    try:
-        out["power_limit"] = subprocess.check_output(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"], text=True).strip()
-    except Exception:
-        out["power_limit"] = None
-    for k in (0, args.k):
-        env.set_subtask(k)
+    def timed(key, k):
         env.reset()  # warm-up: module load, and the first reset from creation state
         ms = []
         for _ in range(args.repeats):
@@ -45,8 +43,22 @@ def main():
             b.synchronize()
             ms.append(a.elapsed_time(b))
         ms.sort()
-        out["k%d_ms" % k] = {"median": ms[len(ms) // 2], "min": ms[0], "max": ms[-1]}
+        out[key] = {"median": ms[len(ms) // 2], "min": ms[0], "max": ms[-1]}
         assert int(env.engine.get("num_connected").min()) == k
+
+    for k in (0, args.k):
+        env.set_subtask(k)
+        env.set_init_qpos(None)
+        timed("k%d_ms" % k, k)
+        if args.init_state:
+            st = env.get_env_state()
+            env.set_init_qpos({"qpos": st["qpos"][0], "qvel": st["qvel"][0]})
+            timed("init_state_k%d_ms" % k, k)
+    try:  # read right after the timed launches, so that the SM clock is the one they ran at
+        q = subprocess.check_output(["nvidia-smi", "--query-gpu=power.limit,clocks.sm", "--format=csv,noheader", "-i", "0"], text=True).strip()
+        out["power_limit"], out["sm_clock_after"] = [x.strip() for x in q.split(",")]
+    except Exception:
+        out["power_limit"] = out["sm_clock_after"] = None
     print(json.dumps(out))
 
 
