@@ -15,6 +15,13 @@
 #define FE_MAXCONN 48
 #define FE_INFO_DIM 6
 
+// the observation flags of config/furniture.py (robot_ob, object_ob, object_ob_all, subtask_ob; read at furniture.py:103-107) as the bits of
+// fe_scene.obs_layout, each set where the flag differs from its default, so that 0 is the default row [object_ob (7 per part) | robot_ob]
+#define FE_OBS_NO_ROBOT 1      /* robot_ob = False */
+#define FE_OBS_NO_OBJECT 2     /* object_ob = False */
+#define FE_OBS_PAIR_ONLY 4     /* object_ob_all = False: object_ob holds the two parts of the current subtask, 14 numbers */
+#define FE_OBS_SUBTASK 8       /* subtask_ob = True: [part1 + 1, part2 + 1] after object_ob */
+
 typedef struct fe_scene {
   int32_t magic, struct_bytes;
   int32_t obs_dim, act_dim, robot_ob_dim, nconn, npart, narm, ngrip; // narm / ngrip: arm / gripper joints of all arms together
@@ -35,7 +42,8 @@ typedef struct fe_scene {
   int32_t arm_dof[FE_MAXRDOF], grip_dof[8];
   float robot_init_qpos[FE_MAXRDOF]; // arm joints (arm_dof order), then gripper joints (grip_dof order)
   float part_init_pos[FE_MAXPART][3], part_init_quat[FE_MAXPART][4], part_radius[FE_MAXPART];
-  int32_t phase_ob, pad_;      // 1: obs ends with the 8-way one-hot of the dense reward's phase (furniture_sawyer_dense.py:100-117); counted in obs_dim
+  int32_t phase_ob;            // 1: obs ends with the 8-way one-hot of the dense reward's phase (furniture_sawyer_dense.py:100-117); counted in obs_dim
+  int32_t obs_layout;          // FE_OBS_* bits of fe_set_obs_layout; 0 = the reference's default flags, the layout of a scene file
   fe_dense_recipe dense;       // assembly recipe for the dense reward (nsub = 0: the furniture has none)
 } fe_scene;
 
@@ -47,6 +55,7 @@ struct FeEnvState {
   int *num_connected, *prev_num_connected, *touched, *picked, *episode_len, *done;
   int *preassembled, *num_connects;            // [N] set_subtask (furniture.py:204-207): recipe steps connected by the env's next reset; connections asked for, -1 = None
   int* success_num_conn;                       // [N] _success_num_conn as the env's last reset left it (furniture.py:1477-1481)
+  int* subtask_part;                           // [N][2] _subtask_part1 / _subtask_part2, -1 = none left (furniture.py:2723-2736)
   uint32_t* mt;                                // [N][624] MT19937 state of the env's numpy RandomState(seed + env)
   int* mt_pos;                                 // [N] position in the state (624 = regenerate before the next draw)
   // recorded starts, _init_qpos (furniture.py:121-130, :315-316, :1433-1434): a bank shared by the envs, and per env the entry its resets start from
@@ -266,6 +275,7 @@ struct FeEnvScratchI {
   int site1, site2;      // sites of the aligned pair
   int conn1, conn2;      // their connector indices
   int done;              // the step ends the episode: auto-reset
+  int dense_pair;        // the dense reward moved on to its next subtask during this step: its recipe pair replaces subtask_part after the observation
 };
 struct FeEnv {
   FeWarp* w;      // header of the env's slice
@@ -281,6 +291,24 @@ struct FeEnv {
 };
 
 FE_HD int fe_find(int* g, int i) { while (g[i] != i) i = g[i]; return i; } // path compression does not change results
+
+// _get_next_subtask (furniture.py:2723-2736), lane 0: the first weld in model order whose two parts lie in different groups (_find_group,
+// :2738-2747), -1 / -1 when there is none.  The reference calls it at the end of every _connect (:917) and of _reset (:1653).
+FE_HD void fe_next_subtask(FeEnv* e) {
+  const fe_scene* sc = e->sc;
+  int p1 = -1, p2 = -1;
+  for (int q = 0; q < e->w->m->neq; ++q)
+    if (fe_find(e->group, sc->eq_part1[q]) != fe_find(e->group, sc->eq_part2[q])) { p1 = sc->eq_part1[q]; p2 = sc->eq_part2[q]; break; }
+  e->es.subtask_part[2 * e->env] = p1;
+  e->es.subtask_part[2 * e->env + 1] = p2;
+}
+// FurnitureSawyerDenseRewardEnv._update_reward_variables (furniture_sawyer_dense.py:149-162), lane 0: the pair becomes recipe step s's (leg, table).
+// The table is the part that carries the step's table site.
+FE_HD void fe_dense_subtask_pair(FeEnv* e, int s) {
+  const fe_model* m = e->w->m;
+  e->es.subtask_part[2 * e->env] = e->sc->dense.leg_part[s];
+  e->es.subtask_part[2 * e->env + 1] = m->site_link[e->sc->dense.table_site[s]] - m->nrlink;
+}
 
 // site world pose (float64) from the link poses of the last forward pass held in the warp slice
 FE_HDN void fe_site_pose_d(const FeWarp* w, int site, double* pos, double* mat, double* quat) {
@@ -486,6 +514,7 @@ FE_FN void fe_connect(FeEnv* e, int align) {
         }
       }
       e->es.num_connected[e->env] += 1;
+      fe_next_subtask(e);   // :917
       e->si->repin = body1; // _connected_body1 and its pose
       const int qa = m->link_qadr[m->nrlink + body1];
       for (int k = 0; k < 7; ++k) e->sd->body1_pose[k] = (double)w->qpos()[qa + k];
@@ -493,11 +522,70 @@ FE_FN void fe_connect(FeEnv* e, int align) {
   LANES_END
 }
 
-// _get_obs: object_ob (7 per part, XML order) then robot_ob (furniture.py:1344-1387, furniture_sawyer.py:103-155)
+// robot_ob of every arm from rb on, by every lane: per arm qpos, qvel, gripper qpos, eef pos, quat (xyzw), velp, velr (furniture_sawyer.py:103-155,
+// furniture_baxter.py:98-155)
+FE_HD void fe_write_robot_ob(FeEnv* e, float* rb, int lane) {
+  FeWarp* w = e->w;
+  const fe_model* m = w->m;
+  const fe_scene* sc = e->sc;
+  const int nar = sc->narms > 0 ? sc->narms : 1, na = sc->narm / nar, ngr = sc->ngrip / nar, per = 2 * na + ngr + 13;
+  for (int arm = 0; arm < sc->narms; ++arm) {
+    float* r = rb + arm * per;
+    for (int d = lane; d < na; d += 32) { const int dof = sc->arm_dof[arm * na + d]; r[d] = w->qpos()[dof]; r[na + d] = w->qvel()[dof]; }
+    for (int d = lane; d < ngr; d += 32) r[2 * na + d] = w->qpos()[sc->grip_dof[arm * ngr + d]];
+    if (lane == 0 && sc->eef_site[arm] >= 0) {
+      float* o = r + 2 * na + ngr;
+      const int s = sc->eef_site[arm], l = m->site_link[s], hl = sc->hand_link[arm];
+      float t[3], sp[3], q[4];
+      m3mulv(t, w->lmat() + 9 * l, m->site_pos[s]);
+      v3add(sp, w->lpos() + 3 * l, t);
+      v3cpy(o, sp);
+      qmul(q, w->lquat() + 4 * hl, sc->hand_quat[arm]);
+      o[3] = q[1]; o[4] = q[2]; o[5] = q[3]; o[6] = q[0]; // xyzw
+      fe_point_vel(w, w->lvel(), l, sp, o + 7);
+      v3cpy(o + 10, w->lvel() + 6 * l);
+    }
+  }
+}
+
+// _get_obs under the flags of fe_set_obs_layout (furniture.py:1344-1387): the row [object_ob | subtask_ob | robot_ob | phase_ob], each entry present
+// as its flag asks.  It shows the subtask pair held in subtask_part, which the step's dense reward has not moved yet.
+FE_FN void fe_write_obs_layout(FeEnv* e) {
+  FeWarp* w = e->w;
+  const fe_model* m = w->m;
+  const fe_scene* sc = e->sc;
+  const int lay = sc->obs_layout, nrl = m->nrlink, np = m->npart;
+  const int* pair = e->es.subtask_part + 2 * e->env;
+  const bool all = !(lay & (FE_OBS_NO_OBJECT | FE_OBS_PAIR_ONLY)), two = (lay & (FE_OBS_NO_OBJECT | FE_OBS_PAIR_ONLY)) == FE_OBS_PAIR_ONLY;
+  const int nobj = all ? 7 * np : (two ? 14 : 0), nsub = (lay & FE_OBS_SUBTASK) ? 2 : 0;
+  float* ob = e->es.obs + (size_t)e->env * sc->obs_dim;
+  for (int pass = 0; pass < (e->es.packed ? 2 : 1); ++pass) {
+  if (pass == 1) ob = e->es.packed + (size_t)e->env * (sc->obs_dim + 2);
+  LANES_BEGIN
+    const int p1 = pair[0], p2 = pair[1];
+    if (all) {
+      for (int p = lane; p < np; p += 32) {
+        for (int k = 0; k < 3; ++k) ob[7 * p + k] = w->lpos()[3 * (nrl + p) + k];
+        for (int k = 0; k < 4; ++k) ob[7 * p + 3 + k] = w->lquat()[4 * (nrl + p) + k];
+      }
+    } else if (two && lane < 14) { // the loop over _object_names keeps the pair's parts in part order; none left: np.zeros(14) (:1364-1375)
+      const int p = lane < 7 ? (p1 < p2 ? p1 : p2) : (p1 < p2 ? p2 : p1), k = lane % 7;
+      ob[lane] = p1 < 0 ? 0.f : (k < 3 ? w->lpos()[3 * (nrl + p) + k] : w->lquat()[4 * (nrl + p) + k - 3]);
+    }
+    if (nsub && lane < 2) ob[nobj + lane] = (float)((lane == 0 ? p1 : p2) + 1); // [_subtask_part1 + 1, _subtask_part2 + 1] (:1379-1382)
+    if (!(lay & FE_OBS_NO_ROBOT)) fe_write_robot_ob(e, ob + nobj + nsub, lane);
+    if (sc->phase_ob && lane < 8) ob[sc->obs_dim - 8 + lane] = (e->es.dstate && e->es.dstate[e->env].phase == lane) ? 1.f : 0.f;
+  LANES_END
+  }
+}
+
+// _get_obs: object_ob (7 per part, XML order) then robot_ob (furniture.py:1344-1387, furniture_sawyer.py:103-155); the other flags' rows are
+// fe_write_obs_layout's
 FE_FN void fe_write_obs(FeEnv* e) {
   FeWarp* w = e->w;
   const fe_model* m = w->m;
   const fe_scene* sc = e->sc;
+  if (sc->obs_layout) { fe_write_obs_layout(e); return; }
   float* ob = e->es.obs + (size_t)e->env * sc->obs_dim;
   const int nrl = m->nrlink, np = m->npart;
   for (int pass = 0; pass < (e->es.packed ? 2 : 1); ++pass) {
@@ -507,25 +595,7 @@ FE_FN void fe_write_obs(FeEnv* e) {
       for (int k = 0; k < 3; ++k) ob[7 * p + k] = w->lpos()[3 * (nrl + p) + k];
       for (int k = 0; k < 4; ++k) ob[7 * p + 3 + k] = w->lquat()[4 * (nrl + p) + k];
     }
-    float* rb = ob + 7 * np;
-    const int nar = sc->narms > 0 ? sc->narms : 1, na = sc->narm / nar, ngr = sc->ngrip / nar, per = 2 * na + ngr + 13; // per arm: qpos, qvel, gripper, eef pos, quat, velp, velr
-    for (int arm = 0; arm < sc->narms; ++arm) {
-      float* r = rb + arm * per;
-      for (int d = lane; d < na; d += 32) { const int dof = sc->arm_dof[arm * na + d]; r[d] = w->qpos()[dof]; r[na + d] = w->qvel()[dof]; }
-      for (int d = lane; d < ngr; d += 32) r[2 * na + d] = w->qpos()[sc->grip_dof[arm * ngr + d]];
-      if (lane == 0 && sc->eef_site[arm] >= 0) {
-        float* o = r + 2 * na + ngr;
-        const int s = sc->eef_site[arm], l = m->site_link[s], hl = sc->hand_link[arm];
-        float t[3], sp[3], q[4];
-        m3mulv(t, w->lmat() + 9 * l, m->site_pos[s]);
-        v3add(sp, w->lpos() + 3 * l, t);
-        v3cpy(o, sp);
-        qmul(q, w->lquat() + 4 * hl, sc->hand_quat[arm]);
-        o[3] = q[1]; o[4] = q[2]; o[5] = q[3]; o[6] = q[0]; // xyzw
-        fe_point_vel(w, w->lvel(), l, sp, o + 7);
-        v3cpy(o + 10, w->lvel() + 6 * l);
-      }
-    }
+    fe_write_robot_ob(e, ob + 7 * np, lane);
     if (sc->phase_ob && lane < 8) ob[sc->obs_dim - 8 + lane] = (e->es.dstate && e->es.dstate[e->env].phase == lane) ? 1.f : 0.f;
   LANES_END
   }
@@ -699,9 +769,11 @@ FE_FN void fe_env_reset_sync(FeEnv* e, int pre) {
     if (lane == 0) {
       e->es.done[e->env] = 0;
       e->si->repin = -1; // _connected_body1 = None (:1558): the preassembly leaves no re-pin pending
+      fe_next_subtask(e); // :1653, after the preassembly in both branches
       if (e->es.dense) { // FurnitureSawyerDenseRewardEnv._reset: _reset_reward_variables on the settled scene
         FeSliceWorld world = {w};
         fe_dense_begin_episode(world, e->es.dense, &sc->dense, pre, e->es.dstate + e->env); // dense_info keeps the last step's terms (the terminal step's, after an auto-reset)
+        fe_dense_subtask_pair(e, pre);
       }
     }
   LANES_END
@@ -864,6 +936,7 @@ FE_HD void fe_env_finish(FeEnv* e, const float* a, int act_dim, float connect, i
       const int n_goal = e->es.success_num_conn[env];
       int success = (nc == n_goal && np > 1) ? 1 : 0;
       int done = success;
+      e->si->dense_pair = 0;
       if (e->es.dense) { // FurnitureSawyerEnv._step: reward, _done, info = _compute_reward(a); done = done or _done (furniture_sawyer.py:66-84)
         FeSliceWorld world = {w};
         const double thr[4] = {cfg->alignment_pos_dist, cfg->alignment_rot_dist_up, cfg->alignment_rot_dist_forward, cfg->alignment_project_dist};
@@ -871,7 +944,9 @@ FE_HD void fe_env_finish(FeEnv* e, const float* a, int act_dim, float connect, i
         for (int k = 0; k < act_dim; ++k) ad[k] = (double)a[k];
         int dd = 0;
         FeDenseState* ds = e->es.dstate + env;
+        const int sub0 = ds->subtask;
         fe_dense_step(world, e->es.dense, &sc->dense, thr, n_goal, ds, ad, act_dim, connected_now, &dr, &dd, di);
+        e->si->dense_pair = ds->subtask != sub0 && !ds->success; // _set_next_subtask moved on without finishing (furniture_sawyer_dense.py:141-147)
         reward = (float)dr;
         success = ds->success;
         done = done || dd;
@@ -895,7 +970,14 @@ FE_HD void fe_env_finish(FeEnv* e, const float* a, int act_dim, float connect, i
       e->si->done = done;
     }
   LANES_END
-  if (e->si->done) fe_env_reset_one(e); else fe_write_obs(e);
+  if (e->si->done) {
+    fe_env_reset_one(e);
+  } else {
+    fe_write_obs(e);
+    // FurnitureSawyerEnv._step takes the observation before _compute_reward (furniture_sawyer.py:66-84): it shows the pair as the connect scan
+    // left it, and the dense reward's new subtask pair is the env's from here on
+    LANES_BEGIN if (lane == 0 && e->si->dense_pair) fe_dense_subtask_pair(e, e->es.dstate[env].subtask); LANES_END
+  }
 }
 
 // FurnitureEnv.step for one env; writes reward / done / info; auto-resets when done (subproc_vec_env.py:16-20)

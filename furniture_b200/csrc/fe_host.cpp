@@ -287,6 +287,12 @@ static int plat_step_host(fe_handle* h, const float* actions, float* obs, float*
   if (int rc = plat_prepare(h)) return rc;
   CudaPlat* p = (CudaPlat*)h->plat;
   const size_t N = h->N, ab = sizeof(float) * N * fe_action_dim(h), ob = sizeof(float) * N * h->hs.obs_dim, rb = sizeof(float) * N, ib = sizeof(int32_t) * N * FE_INFO_DIM;
+  if (ob + rb + ib + N != p->out_bytes) { // fe_set_obs_layout changed obs_dim after the staging was sized
+    CUDA_OK(cudaFreeHost(p->pin_out));
+    p->pin_out = nullptr;
+    p->out_bytes = ob + rb + ib + N;
+    CUDA_OK(cudaMallocHost((void**)&p->pin_out, p->out_bytes + 64));
+  }
   memcpy(p->pin_act, actions, ab);
   // The private stream is ordered behind whatever the caller last launched for this handle on another stream
   // (fe_sim_forward, fe_env_reset ...) with an event, not with a device-wide synchronisation.

@@ -30,6 +30,8 @@ STAT_WAIT_KIN, STAT_WAIT_COLLIDE, STAT_WAIT_ASSEMBLE, STAT_WAIT_SOLVE, STAT_WAIT
 STAT_SOLVE_PRE, STAT_SOLVE_GROUPED, STAT_SOLVE_COMP, STAT_RESERVED = 17, 18, 19, 20
 STAT_NEWTON_SETUP, STAT_NEWTON_START, STAT_NEWTON_GRAD, STAT_NEWTON_HESSIAN, STAT_NEWTON_CHOL, STAT_NEWTON_PRODUCTS, STAT_NEWTON_LS = 21, 22, 23, 24, 25, 26, 27
 i32, f32, f64 = C.c_int32, C.c_float, C.c_double
+# the observation flags of config/furniture.py:228-258 and their defaults; other values go to fe_set_obs_layout
+OBS_DEFAULTS = dict(robot_ob=True, object_ob=True, object_ob_all=True, subtask_ob=False)
 
 
 class FeConfig(C.Structure):
@@ -55,7 +57,7 @@ class FeScene(C.Structure):
         ("arm_dof", i32 * MAXRDOF), ("grip_dof", i32 * 8),
         ("robot_init_qpos", f32 * MAXRDOF),
         ("part_init_pos", (f32 * 3) * MAXPART), ("part_init_quat", (f32 * 4) * MAXPART), ("part_radius", f32 * MAXPART),
-        ("phase_ob", i32), ("pad_", i32), ("dense", FeDenseRecipe),
+        ("phase_ob", i32), ("obs_layout", i32), ("dense", FeDenseRecipe),
     ]
 
 
@@ -191,9 +193,35 @@ def build_scene(m: mjcf.Model, em: EngineModel, phase_ob: bool = False) -> FeSce
     return sc
 
 
+def obs_columns(scene, robot_skip=0, robot_ob=True, object_ob=True, object_ob_all=True, subtask_ob=False):
+    """Where each entry of the obs dict sits in a device row, in the reference's key order: object_ob, subtask_ob (FurnitureEnv._get_obs,
+    furniture.py:1344-1387), robot_ob (the agent's, furniture_sawyer.py:103-155, furniture_baxter.py:98-155), phase_ob (the dense env's).
+    An OrderedDict of key -> slice, or of index array for the robot_ob of two arms that drop their `robot_skip` joint columns each (the IK and
+    controller control types, furniture_baxter.py:137-160)."""
+    from collections import OrderedDict
+
+    cols, o = OrderedDict(), 0
+    if object_ob:
+        w = 7 * scene.npart if object_ob_all else 14
+        cols["object_ob"], o = slice(o, o + w), o + w
+    if subtask_ob:
+        cols["subtask_ob"], o = slice(o, o + 2), o + 2
+    if robot_ob:
+        narms, dim = max(1, int(scene.narms)), int(scene.robot_ob_dim)
+        per = dim // narms
+        if robot_skip and narms > 1:
+            cols["robot_ob"] = np.array([o + a * per + k for a in range(narms) for k in range(robot_skip, per)])
+        else:
+            cols["robot_ob"] = slice(o + robot_skip, o + dim)
+        o += dim
+    if scene.phase_ob:
+        cols["phase_ob"], o = slice(o, o + 8), o + 8
+    return cols
+
+
 class Engine:
     def __init__(self, model: mjcf.Model, n_envs: int, device: int = 0, config: FeConfig | None = None, lib_path: str | None = None,
-                 dense: FeDenseConfig | None = None, ik=None, controller=None):
+                 dense: FeDenseConfig | None = None, ik=None, controller=None, obs_layout=None):
         path = lib_path or DEFAULT_LIB
         if not os.path.exists(path):
             raise RuntimeError(
@@ -236,6 +264,9 @@ class Engine:
         if controller is not None:  # one of the NEW_CONTROLLERS (furniture_b200/controllers.py: FeCtlConfig) on the torque-actuated robot
             self._chk(L.fe_enable_controller(self.h, C.byref(controller)))
             self.act_dim = int(L.fe_action_dim(self.h))
+        self.obs_flags = dict(OBS_DEFAULTS)
+        if obs_layout is not None and {**OBS_DEFAULTS, **obs_layout} != OBS_DEFAULTS:  # `obs_layout`: overrides of OBS_DEFAULTS
+            self.set_obs_layout(**obs_layout)
         self._bank, self._n_pick = [], 0  # host copy of the bank of recorded starts; its first _n_pick entries are the load_init_states list
         self.dense = dense
         if dense is not None:  # FurnitureSawyerDenseRewardEnv: the phase machine replaces the sparse reward inside fe_env_step
@@ -264,7 +295,7 @@ class Engine:
 
     _INT = {"order", "geom_contype", "geom_conaffinity", "eq_active", "touch", "flags", "ncon", "niter", "stats", "con_geom", "con_state", "group", "site_connected",
             "num_connected", "prev_num_connected", "touched", "picked", "episode_length", "done", "mt_pos", "preassembled", "num_connects",
-            "init_state", "init_pick", "init_mt_pos"}
+            "init_state", "init_pick", "init_mt_pos", "subtask_part"}
     _U32 = {"mt_state", "init_mt_state"}
 
     def get(self, name):
@@ -321,6 +352,14 @@ class Engine:
         self._chk(self.L.fe_env_step_host(self.h, a.ctypes.data_as(C.c_void_p), obs.ctypes.data_as(C.c_void_p), rew.ctypes.data_as(C.c_void_p),
                                           done.ctypes.data_as(C.c_void_p), info.ctypes.data_as(C.c_void_p)))
         return obs, rew, done, info
+
+    def set_obs_layout(self, robot_ob=True, object_ob=True, object_ob_all=True, subtask_ob=False):
+        """fe_set_obs_layout: the observation flags of config/furniture.py (furniture.py:103-107), before the first reset"""
+        flags = dict(robot_ob=robot_ob, object_ob=object_ob, object_ob_all=object_ob_all, subtask_ob=subtask_ob)
+        self._chk(self.L.fe_set_obs_layout(self.h, *[int(v) if isinstance(v, (bool, np.bool_)) else v for v in flags.values()]))
+        self.obs_flags = {k: bool(v) for k, v in flags.items()}
+        self.obs_dim = self.scene.obs_dim = int(self.L.fe_obs_dim(self.h))
+        self.scene.obs_layout = (0 if robot_ob else 1) | (0 if object_ob else 2) | (0 if object_ob_all else 4) | (8 if subtask_ob else 0)
 
     def set_max_episode_steps(self, n):
         self._chk(self.L.fe_set_max_episode_steps(self.h, int(n)))

@@ -18,7 +18,7 @@ import numpy as np
 
 from . import mjcf
 from .dense import DENSE_DEFAULTS, DENSE_ENV_DEFAULTS, INFO_KEYS as DENSE_INFO_KEYS, dense_config
-from .engine import INFO_DIM, Engine, default_config
+from .engine import INFO_DIM, OBS_DEFAULTS, Engine, default_config, obs_columns
 
 INFO_KEYS = ("num_connected", "episode_success", "episode_unstable", "episode_length", "ncon", "solver_iters")
 ENV_IDS = {"IKEASawyer-v0": "Sawyer", "FurnitureSawyerEnv": "Sawyer", "IKEABaxter-v0": "Baxter", "FurnitureBaxterEnv": "Baxter",
@@ -51,8 +51,9 @@ def split_config(config):
     """Reference-style config (argparse Namespace or dict, config/furniture.py) -> (furniture name, FeConfig overrides, ignored keys).
     `furniture_name` wins over `furniture_id` as in furniture.py:157-161; keys the accelerated path has no use for (port, background,
     camera and rendering options ...) are returned so that callers can report them instead of failing on them.  `preassembled` (checked to be
-    a recipe prefix), `num_connects`, `load_init_states` and `load_demo` travel with the overrides when they are set: they are keywords of the
-    env constructors."""
+    a recipe prefix), `num_connects`, `load_init_states`, `load_demo` and the observation flags `robot_ob`, `object_ob`, `object_ob_all`,
+    `subtask_ob` travel with the overrides when they are set (the flags when they differ from their defaults): they are keywords of the env
+    constructors."""
     from .engine import FeConfig
 
     cfg = dict(vars(config)) if hasattr(config, "__dict__") and not isinstance(config, dict) else dict(config or {})
@@ -68,7 +69,7 @@ def split_config(config):
     renamed = {"furn_xyz_rand": "furn_xyz_rand", "furn_rot_rand": "furn_rot_rand", "agent_xyz_rand": "agent_xyz_rand", "alignment_pos_dist": "alignment_pos_dist"}
     over = {renamed.get(k, k): v for k, v in cfg.items() if renamed.get(k, k) in fields and v is not None}
     ignored = sorted(k for k in cfg if k not in over and k not in ("furniture_name", "furniture_id", "control_type", "preassembled", "num_connects",
-                                                                   "load_init_states", "load_demo"))
+                                                                   "load_init_states", "load_demo") + tuple(OBS_DEFAULTS))
     if prefix_length(cfg.get("preassembled")):
         over["preassembled"] = list(cfg["preassembled"])
     if cfg.get("num_connects") is not None:
@@ -76,6 +77,9 @@ def split_config(config):
     for k in ("load_init_states", "load_demo"):  # paths of pickles (furniture.py:121-130), read by the env constructors
         if cfg.get(k):
             over[k] = cfg[k]
+    for k, default in OBS_DEFAULTS.items():  # furniture.py:103-107; a flag at its default changes nothing and is not passed on
+        if cfg.get(k) is not None and bool(cfg[k]) != default:
+            over[k] = bool(cfg[k])
     return name or "table_lack_0825", over, ignored
 
 
@@ -120,7 +124,8 @@ def apply_init_config(env, load_init_states=None, load_demo=None):
 
 class BatchedFurnitureEnv:
     def __init__(self, agent="Sawyer", furniture_name="table_lack_0825", num_envs=1, device=0, dense=None, control_type="impedance", ik=None,
-                 preassembled=None, num_connects=None, load_init_states=None, load_demo=None, **cfg_overrides):
+                 preassembled=None, num_connects=None, load_init_states=None, load_demo=None, robot_ob=True, object_ob=True, object_ob_all=True,
+                 subtask_ob=False, **cfg_overrides):
         """`dense`: None for the sparse reward of FurnitureEnv; a dict of coefficient overrides (possibly empty) for the phase-based
         reward of FurnitureSawyerDenseRewardEnv, computed inside the step kernel (furniture_b200/dense.py).
         `control_type`: "impedance" (joint velocities, dof 9), "ik" (move 3, rotate 3, gripper, connect: dof 8) or "ik_quaternion" (the
@@ -132,7 +137,10 @@ class BatchedFurnitureEnv:
         `preassembled`, `num_connects`: config/furniture.py:81, :158 -- the recipe prefix [0, ..., k-1] every env starts its episodes
         from and the connections that end one; set_subtask changes them per env later.
         `load_init_states`, `load_demo`: config/furniture.py's paths (furniture.py:121-130), or the states themselves: every env picks its
-        starts from the list of `load_init_states` (see load_init_states), and every env starts from the first state of the demo `load_demo`."""
+        starts from the list of `load_init_states` (see load_init_states), and every env starts from the first state of the demo `load_demo`.
+        `robot_ob`, `object_ob`, `object_ob_all`, `subtask_ob`: the observation flags of config/furniture.py (furniture.py:103-107, :215-252,
+        :1344-1387).  object_ob_all=False keeps in object_ob only the two parts of each env's current subtask (14 numbers, zeros when none is
+        left); subtask_ob=True adds their part ids + 1 (float32).  Each env's pair follows its connections and resets inside the kernels."""
         import torch
 
         if not torch.cuda.is_available():
@@ -170,23 +178,21 @@ class BatchedFurnitureEnv:
             self.ctl_cfg = ctl_config(control_type, model=self.model, move_speed=(ik or {}).get("move_speed", 0.1))
         elif control_type not in ("impedance", "ik", "ik_quaternion"):
             raise NotImplementedError("control_type %r is not built" % control_type)
-        self.engine = Engine(self.model, num_envs, device=device, config=self.cfg, dense=self.dense_cfg, ik=self.ik_cfg, controller=self.ctl_cfg)
+        self.obs_flags = dict(robot_ob=bool(robot_ob), object_ob=bool(object_ob), object_ob_all=bool(object_ob_all), subtask_ob=bool(subtask_ob))
+        self.engine = Engine(self.model, num_envs, device=device, config=self.cfg, dense=self.dense_cfg, ik=self.ik_cfg, controller=self.ctl_cfg,
+                             obs_layout=self.obs_flags)
         self.num_envs = num_envs
         self.obs_dim, self.act_dim = self.engine.obs_dim, self.engine.act_dim
         self.n_objects = self.engine.scene.npart
-        self.object_ob_dim = 7 * self.n_objects
-        self.robot_ob_dim = self.engine.scene.robot_ob_dim
         # control_type="ik": robot_ob is gripper_qpos, eef_pos, eef_quat, eef_velp, eef_velr only -- no joint positions / velocities
-        # (furniture_sawyer.py:110-125); the device row always holds all of it, the 15 numbers are its tail
+        # (furniture_sawyer.py:110-125); the device row always holds all of it, the 15 numbers are its tail (of each arm's block for two arms,
+        # furniture_baxter.py:137-160)
         self._robot_skip = 0 if control_type == "impedance" else 14
         self._narms = max(1, int(self.engine.scene.narms))
-        self.robot_ob_dim -= self._robot_skip * self._narms
-        self._robot_cols = None
-        if self._robot_skip and self._narms > 1:  # two arms: the 15-number tail of each arm's block (furniture_baxter.py:137-160)
-            per = self.engine.scene.robot_ob_dim // self._narms
-            cols = [self.object_ob_dim + a * per + k for a in range(self._narms) for k in range(self._robot_skip, per)]
-            self._robot_cols = torch.tensor(cols, dtype=torch.long, device=self.device)
-        self.phase_ob_dim = 8 if self.engine.scene.phase_ob else 0
+        self._cols = obs_columns(self.engine.scene, self._robot_skip, **self.obs_flags)
+        width = lambda k: (len(range(self.obs_dim)[self._cols[k]]) if isinstance(self._cols[k], slice) else len(self._cols[k])) if k in self._cols else 0
+        self.object_ob_dim, self.subtask_ob_dim, self.robot_ob_dim, self.phase_ob_dim = (width(k) for k in ("object_ob", "subtask_ob", "robot_ob", "phase_ob"))
+        self._cols = OrderedDict((k, c if isinstance(c, slice) else torch.tensor(c, dtype=torch.long, device=self.device)) for k, c in self._cols.items())
         self.dof = self.act_dim
         self._obs = torch.empty((num_envs, self.obs_dim), dtype=torch.float32, device=self.device)
         self._rew = torch.empty(num_envs, dtype=torch.float32, device=self.device)
@@ -226,24 +232,21 @@ class BatchedFurnitureEnv:
     # spaces, in the reference's terms (furniture.py:215-252, :293-310)
     @property
     def observation_space(self):
-        sp = OrderedDict(object_ob=(self.object_ob_dim,), robot_ob=(self.robot_ob_dim,))
-        if self.phase_ob_dim:
-            sp["phase_ob"] = (8,)  # furniture_sawyer_dense.py:100-109
-        return sp
+        """key -> shape, in the order of the obs dict: object_ob (7 n_objects, or 14), subtask_ob (2), robot_ob, phase_ob (8, furniture_sawyer_dense.py:100-109)"""
+        widths = dict(object_ob=self.object_ob_dim, subtask_ob=self.subtask_ob_dim, robot_ob=self.robot_ob_dim, phase_ob=self.phase_ob_dim)
+        return OrderedDict((k, (widths[k],)) for k in self._cols)
 
     @property
     def action_space(self):
         return OrderedDict(default=(self.act_dim,))
 
     def _obs_dict(self, obs):
-        a, b = self.object_ob_dim, self.object_ob_dim + self._robot_skip * self._narms + self.robot_ob_dim
-        if self._robot_cols is not None:
-            cols = self._robot_cols if hasattr(obs, "index_select") else self._robot_cols.cpu().numpy()
-            d = OrderedDict(object_ob=obs[:, :a], robot_ob=obs.index_select(1, cols) if hasattr(obs, "index_select") else obs[:, cols])
-        else:
-            d = OrderedDict(object_ob=obs[:, :a], robot_ob=obs[:, a + self._robot_skip : b])
-        if self.phase_ob_dim:
-            d["phase_ob"] = obs[:, b:]
+        d = OrderedDict()
+        for k, c in self._cols.items():  # views of the row, but for the two-arm robot_ob without its joint columns
+            if isinstance(c, slice):
+                d[k] = obs[:, c]
+            else:
+                d[k] = obs.index_select(1, c) if hasattr(obs, "index_select") else obs[:, c.cpu().numpy()]
         return d
 
     def dense_infos(self):
@@ -323,7 +326,9 @@ class MixedFurnitureEnv:
     furniture (SURVEY.md 8e: "bucket by furniture id first"): one engine handle per model, each with its own instance of the
     kernels (its own slice-layout table, see csrc/fe_host.cpp) and its own CUDA stream, so the buckets of a step run
     concurrently and fill the SMs together; the caller's stream waits for all of them at the end of the call.
-    nq / nv / obs_dim differ per bucket; `object_ob` is returned zero-padded to the widest model, `robot_ob` is common.
+    nq / nv / obs_dim differ per bucket; `object_ob` is returned zero-padded to the widest model, `robot_ob` is common.  With
+    object_ob_all=False (a keyword passed on to every bucket, like the other observation flags) `object_ob` holds the two parts of each
+    env's current subtask: 14 numbers whatever the model, so nothing is padded; `subtask_ob` (subtask_ob=True) is gathered like the rest.
 
       env = MixedFurnitureEnv(["table_lack_0825", "chair_ingolf_0650"], envs_per_model=64)
       obs = env.reset(); obs, rew, done, info = env.step(actions)          # actions: (num_envs, dof)
@@ -349,11 +354,15 @@ class MixedFurnitureEnv:
         self.device, self.act_dim, self.dof, self.robot_ob_dim = b0.device, b0.act_dim, b0.act_dim, b0.robot_ob_dim
         assert all(b.act_dim == self.act_dim and b.robot_ob_dim == self.robot_ob_dim for b in self.buckets)
         # object_ob is zero-padded to the widest model of this batch, or to `object_ob_dim` (the widest of a sharded batch, so
-        # that every rank's rows have the same width)
-        self.object_ob_dim = max([b.object_ob_dim for b in self.buckets] + [object_ob_dim or 0])
-        self.obs_dim = self.object_ob_dim + self.robot_ob_dim
-        self._obs = torch.zeros((off, self.obs_dim), dtype=torch.float32, device=self.device)  # [object_ob (padded) | robot_ob]
-        self._object_ob, self._robot_ob = self._obs[:, : self.object_ob_dim], self._obs[:, self.object_ob_dim :]
+        # that every rank's rows have the same width); without object_ob_all it is 14 wide everywhere
+        space = b0.observation_space
+        self.object_ob_dim = max([b.object_ob_dim for b in self.buckets] + [object_ob_dim or 0]) if b0.obs_flags["object_ob"] else 0
+        widths = OrderedDict((k, self.object_ob_dim if k == "object_ob" else space[k][0]) for k in space)
+        self.obs_dim = sum(widths.values())
+        self._obs = torch.zeros((off, self.obs_dim), dtype=torch.float32, device=self.device)  # [object_ob (padded) | subtask_ob | robot_ob]
+        self._views, o = OrderedDict(), 0
+        for k, w in widths.items():
+            self._views[k], o = self._obs[:, o : o + w], o + w
         self._rew = torch.empty(off, dtype=torch.float32, device=self.device)
         self._done = torch.empty(off, dtype=torch.uint8, device=self.device)
         self._info = torch.empty((off, INFO_DIM), dtype=torch.int32, device=self.device)
@@ -361,7 +370,10 @@ class MixedFurnitureEnv:
         self._streams = [torch.cuda.Stream(device=self.device) for _ in self.buckets]
 
     def _obs_dict(self, obs):
-        return OrderedDict(object_ob=obs[:, : self.object_ob_dim], robot_ob=obs[:, self.object_ob_dim :])
+        d, o = OrderedDict(), 0
+        for k, v in self._views.items():
+            d[k], o = obs[:, o : o + v.shape[1]], o + v.shape[1]
+        return d
 
     def algorithmic_bytes_per_step(self, nsub=50):
         """SURVEY.md 8d: sum over the buckets of envs x (nsub x 4 (2 nq + 5 nv + nu) + 4 (obs + act) + 8)"""
@@ -387,8 +399,8 @@ class MixedFurnitureEnv:
 
     def _collect(self, b, off, od):
         sl = slice(off, off + b.num_envs)
-        self._object_ob[sl, : b.object_ob_dim].copy_(od["object_ob"])
-        self._robot_ob[sl].copy_(od["robot_ob"])
+        for k, v in od.items():
+            self._views[k][sl, : v.shape[1]].copy_(v)
         return sl
 
     def reset(self):

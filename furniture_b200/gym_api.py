@@ -2,7 +2,7 @@
 `FurnitureGym` (furniture/env/furniture_gym.py:11-80) and of `FurnitureEnv.step()/reset()` behind it.
 
   env = FurnitureGymB200(name="FurnitureSawyerEnv", furniture_name="table_lack_0825", seed=123)
-  ob = env.reset()                                  # OrderedDict(object_ob (7 n_objects,), robot_ob (29,))
+  ob = env.reset()                                  # OrderedDict(object_ob (7 n_objects,), robot_ob (29,)); see the observation flags
   ob, reward, done, info = env.step(action)         # action: (dof,) array or {"default": array}
 
 It is the batched engine with one env (the batch entry point `furniture_b200.env.make_vec_env` is the one to use for
@@ -21,7 +21,7 @@ from collections import OrderedDict
 import numpy as np
 
 from . import mjcf
-from .engine import Engine, default_config
+from .engine import OBS_DEFAULTS, Engine, default_config, obs_columns
 
 AGENTS = {"FurnitureSawyerDenseRewardEnv": "Sawyer", "IKEASawyerDense-v0": "Sawyer", "furniture-sawyer-densereward-v0": "Sawyer", "FurnitureSawyerEnv": "Sawyer", "IKEASawyer-v0": "Sawyer", "Sawyer": "Sawyer", "FurnitureBaxterEnv": "Baxter", "IKEABaxter-v0": "Baxter", "Baxter": "Baxter"}
 
@@ -47,6 +47,7 @@ class FurnitureGymB200:
             furniture_name, over, self.ignored_config = split_config(config)
         preassembled, num_connects = prefix_length(over.pop("preassembled", None)), over.pop("num_connects", None)
         load_init_states, load_demo = over.pop("load_init_states", None), over.pop("load_demo", None)
+        self.obs_flags = dict(OBS_DEFAULTS, **{k: over.pop(k) for k in OBS_DEFAULTS if k in over})  # robot_ob ... subtask_ob (furniture.py:103-107)
         ctl = control_options(config)
         self.control_type, self.ik_cfg, self.ctl_cfg = ctl["control_type"], None, None
         agent = AGENTS[name]
@@ -66,16 +67,15 @@ class FurnitureGymB200:
             from .ik import ik_config
 
             self.ik_cfg = ik_config(self.model, **dict(ctl["ik"], quaternion_mode=int(self.control_type == "ik_quaternion")))
-        self.engine = Engine(self.model, 1, device=device, config=self.cfg, lib_path=lib_path, dense=self.dense_cfg, ik=self.ik_cfg, controller=self.ctl_cfg)
+        self.engine = Engine(self.model, 1, device=device, config=self.cfg, lib_path=lib_path, dense=self.dense_cfg, ik=self.ik_cfg, controller=self.ctl_cfg,
+                             obs_layout=self.obs_flags)
         self.n_objects = self.engine.scene.npart
-        self.object_ob_dim = 7 * self.n_objects
-        self.robot_ob_dim = self.engine.scene.robot_ob_dim
-        self.phase_ob_dim = 8 if self.engine.scene.phase_ob else 0
         self._robot_skip = 0 if self.control_type == "impedance" else 14  # ik: robot_ob has no joint positions / velocities (furniture_sawyer.py:110-125)
         self._narms = max(1, int(self.engine.scene.narms))
-        per = self.robot_ob_dim // self._narms
-        self._robot_cols = np.array([self.object_ob_dim + a * per + k for a in range(self._narms) for k in range(self._robot_skip, per)])
-        self.robot_ob_dim -= self._robot_skip * self._narms
+        cols = obs_columns(self.engine.scene, self._robot_skip, **self.obs_flags)
+        self._cols = OrderedDict((k, np.arange(self.engine.obs_dim)[c]) for k, c in cols.items())  # the row's columns of each obs entry
+        width = lambda k: len(self._cols[k]) if k in self._cols else 0
+        self.object_ob_dim, self.subtask_ob_dim, self.robot_ob_dim, self.phase_ob_dim = (width(k) for k in ("object_ob", "subtask_ob", "robot_ob", "phase_ob"))
         self.dof = self.engine.act_dim
         self._max_episode_steps = self.cfg.max_episode_steps
         self._pending_ob = None  # observation of an episode the device has already started
@@ -88,9 +88,7 @@ class FurnitureGymB200:
     # ---- spaces (furniture.py:215-252, :293-310): plain shape / bound records, gym.spaces objects when gym is installed
     @property
     def observation_space(self):
-        shapes = OrderedDict(object_ob=(self.object_ob_dim,), robot_ob=(self.robot_ob_dim,))
-        if self.phase_ob_dim:
-            shapes["phase_ob"] = (8,)
+        shapes = OrderedDict((k, (len(c),)) for k, c in self._cols.items())  # object_ob, subtask_ob, robot_ob, phase_ob as the flags ask
         try:
             import gym.spaces as sp
 
@@ -108,11 +106,7 @@ class FurnitureGymB200:
             return OrderedDict(default=dict(shape=(self.dof,), low=-1.0, high=1.0))
 
     def _ob(self, obs_row):
-        a, b = self.object_ob_dim, self.object_ob_dim + self._robot_skip * self._narms + self.robot_ob_dim
-        ob = OrderedDict(object_ob=obs_row[:a].astype(np.float64), robot_ob=obs_row[self._robot_cols].astype(np.float64))
-        if self.phase_ob_dim:
-            ob["phase_ob"] = obs_row[b:].astype(np.float64)
-        return ob
+        return OrderedDict((k, obs_row[c].astype(np.float64)) for k, c in self._cols.items())
 
     def reset(self):
         if self._pending_ob is not None:

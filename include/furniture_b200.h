@@ -18,6 +18,8 @@
  *   fe_enable_dense_reward <- FurnitureSawyerDenseRewardEnv (env id IKEASawyerDense-v0): _compute_reward and the phase machine
  *                       around it replace the sparse reward inside fe_env_step         furniture_sawyer_dense.py:18-1022
  *   fe_dense_eval    <- the same reward machine on explicit poses (test hook)          furniture_sawyer_dense.py:225-586
+ *   fe_set_obs_layout <- the observation flags robot_ob / object_ob / object_ob_all / subtask_ob, with _get_next_subtask
+ *                       tracked per env inside the kernels    furniture.py:103-107, :215-252, :1344-1387, :2723-2759
  *
  * Conventions: every function returns 0 on success or a negative code and records a message retrievable with
  * fe_last_error(); a handle is bound to one CUDA device, is not thread-safe, and all work is issued on the stream
@@ -84,7 +86,7 @@ void fe_destroy(fe_handle* h);
 const char* fe_last_error(const fe_handle* h); /* h may be NULL: last creation error */
 
 int fe_num_envs(const fe_handle* h);
-int fe_obs_dim(const fe_handle* h);    /* robot_ob (29 for Sawyer impedance) + object_ob (7 per part) */
+int fe_obs_dim(const fe_handle* h);    /* object_ob (7 per part) + robot_ob (29 for Sawyer impedance) by default; see fe_set_obs_layout */
 int fe_action_dim(const fe_handle* h); /* dof: 7 joint velocities + gripper + connect for Sawyer impedance */
 int fe_info_dim(const fe_handle* h);   /* int32 per env: num_connected, success, unstable, episode_length, ncon, solver iters */
 int fe_smem_bytes_per_env(const fe_handle* h); /* shared-memory working set of one env (one warp) */
@@ -100,7 +102,8 @@ int fe_sim_step(fe_handle* h, int nsub, void* stream);
    read/write: FurnitureEnv.set_subtask, furniture.py:204-207.  An env's next reset, an auto-reset included, connects the first `preassembled`
    steps of the scene's assembly recipe before it places the robot, and the episode then succeeds at num_connects + preassembled connections,
    or with every part connected when num_connects is -1); init_state init_pick init_mt_state (624 x uint32) init_mt_pos (int32, one per env,
-   read/write: the env's recorded start, see fe_set_init_states) */
+   read/write: the env's recorded start, see fe_set_init_states); subtask_part (2 x int32 per env, read only: _subtask_part1 / _subtask_part2,
+   the two parts of the env's current subtask, -1 / -1 when none is left -- see fe_set_obs_layout) */
 int fe_get_field(fe_handle* h, const char* name, void* dst_host, size_t bytes);
 int fe_set_field(fe_handle* h, const char* name, const void* src_host, size_t bytes);
 int fe_field_dim(fe_handle* h, const char* name, int* dim, int* elem_bytes);
@@ -180,6 +183,16 @@ int fe_set_max_episode_steps(fe_handle* h, int max_episode_steps);
  * "dense_info" holds (n_envs, fe_dense_info_dim()) float32 per step: phase, subtask, phase_bonus, ctrl_penalty, gripper_penalty,
  * move_other_part_penalty, drop_penalty, touch, drop_leg, table_moved, stable_grip_succ, skips (bit 0 to lift_leg, bit 1 to move_leg_fine). */
 int fe_enable_dense_reward(fe_handle* h, const fe_dense_config* dc);
+/* The observation flags of config/furniture.py (furniture.py:103-107, :215-252, :1344-1387), each 0 or 1; the defaults (1, 1, 1, 0) are the layout
+ * of fe_create.  A row is [object_ob | subtask_ob | robot_ob | phase_ob], each entry present as its flag asks: object_ob holds 7 numbers
+ * (pos, quat wxyz) per part, or with object_ob_all = 0 only those of the two parts of the env's current subtask, in part order (14 numbers,
+ * zeros when no subtask is left); subtask_ob is [part1 + 1, part2 + 1] as float32.  The pair is the reference's _get_next_subtask
+ * (furniture.py:2723-2736): the first weld in model order whose parts are not yet joined, recomputed after every connection and at the end
+ * of every reset; with the dense reward, the recipe step's (leg, table) from each reset and from each move to the next subtask on, which the
+ * observation shows from the following step (the observation of a step is taken before its reward, furniture_sawyer.py:66-84).  Field
+ * "subtask_part" holds the pair.  Call before the first fe_env_reset or env step; it is refused after, and for a flag outside {0, 1}.
+ * fe_obs_dim reports the new width, the obs buffer is reallocated (fe_obs_dev moves), and packed rows keep the stride obs_dim + 2. */
+int fe_set_obs_layout(fe_handle* h, int robot_ob, int object_ob, int object_ob_all, int subtask_ob);
 int fe_dense_info_dim(void);
 /* device pointer of the internal obs buffer after the last step/reset: (n_envs, obs_dim) float32 */
 const float* fe_obs_dev(const fe_handle* h);
