@@ -64,6 +64,12 @@ struct FeEnvState {
   int *init_state, *init_pick;                 // [N] bank index of the env's _init_qpos, -1 = None; leading entries its resets pick from, 0 = no load_init_states
   uint32_t* init_mt;                           // [N][624] MT19937 of the pick, numpy RandomState(seed + 2**20 + env); laid out like mt
   int* init_mt_pos;                            // [N]
+  // fix_init / fix_init_parts (config/furniture.py:116-127): the placement a random-placement reset remembers (furniture.py:1519-1532),
+  // the reference's init_pos / init_quat, and whether it holds one (init_pos is not None)
+  int *fix_init, *fix_init_parts, *fix_have;   // [N] 0 / 1, bit mask over parts in XML order, 0 / 1
+  double* fix_pose;                            // [N][npart][7] position, quaternion (w, x, y, z)
+  int* reset_arm;                              // [N] reset_robot_after_attach (config/furniture.py:169-174)
+  int* arm_resync;                             // [N] a connection sent the arm home: the next IK command re-seeds its position target
   int *robot_contype, *robot_conaff;           // [N][ngeom] saved robot masks during reset
   float* episode_reward;
   // dense (phase-based) reward, fe_dense.h: NULL = the sparse reward of FurnitureEnv._compute_reward
@@ -419,6 +425,18 @@ FE_FN void fe_try_connect_scan(FeEnv* e, int part1) {
 // `align`: FE_ALIGN_CONFIG follows cfg->auto_align (a connection made by the policy); the reset's preassembly passes auto_align=_init_qpos is None
 // (furniture.py:1556): FE_ALIGN_ALWAYS after random placement, FE_ALIGN_NEVER on a recorded start
 enum { FE_ALIGN_CONFIG = 0, FE_ALIGN_ALWAYS = 1, FE_ALIGN_NEVER = 2 };
+// _initialize_robot_pos (furniture.py:1761-1779), lane 0: fresh noise on every call, the arm joints at their start pose plus the noise, the
+// gripper open; qvel untouched.  Called by the reset's robot poses and by fe_connect under reset_robot_after_attach
+FE_HDN void fe_init_robot_pos(FeEnv* e) {
+  FeWarp* w = e->w;
+  const fe_scene* sc = e->sc;
+  uint32_t* mt = e->es.mt + (size_t)e->env * FE_MT_N;
+  int pos = e->es.mt_pos[e->env];
+  const double r = (double)e->cfg->agent_xyz_rand; // _init_random(shape, "agent") = rng.uniform(-r, r, size=7), furniture.py:336-349
+  for (int i = 0; i < sc->narm; ++i) w->qpos()[sc->arm_dof[i]] = (float)ndadd((double)sc->robot_init_qpos[i], fe_mt_uniform(mt, &pos, -r, r));
+  for (int i = 0; i < sc->ngrip; ++i) w->qpos()[sc->grip_dof[i]] = sc->robot_init_qpos[sc->narm + i];
+  e->es.mt_pos[e->env] = pos;
+}
 FE_FN void fe_connect(FeEnv* e, int align) {
   FeWarp* w = e->w;
   const fe_model* m = w->m;
@@ -518,6 +536,7 @@ FE_FN void fe_connect(FeEnv* e, int align) {
       e->si->repin = body1; // _connected_body1 and its pose
       const int qa = m->link_qadr[m->nrlink + body1];
       for (int k = 0; k < 7; ++k) e->sd->body1_pose[k] = (double)w->qpos()[qa + k];
+      if (e->es.reset_arm[e->env]) { fe_init_robot_pos(e); e->es.arm_resync[e->env] = 1; } // :919-924, every _connect (the reset's preassembly too)
     }
   LANES_END
 }
@@ -677,7 +696,9 @@ FE_FN void fe_env_reset_clear(FeEnv* e, int pre) {
     }
   LANES_END
 }
-// _place_objects and the first settle loop (:1519-1540)
+// _place_objects and the first settle loop (:1519-1540).  The env's remembered placement fix_pose is the reference's init_pos / init_quat:
+// with fix_init and a placement held, the parts start there and nothing is drawn (:1522); otherwise the sampler runs and its placement is
+// remembered (:1520-1525), the parts of fix_init_parts planted at their remembered pose and placed first (:1397-1404) once there is one
 FE_FN void fe_env_reset_place(FeEnv* e) {
   FeWarp* w = e->w;
   const fe_model* m = w->m;
@@ -686,19 +707,32 @@ FE_FN void fe_env_reset_place(FeEnv* e) {
   const int nrl = m->nrlink, np = m->npart;
   LANES_BEGIN
     if (lane == 0) { // UniformRandomSampler.sample (placement_sampler.py:137-190): xy noise, z + 0.01, +furn_rot_rand deg about x
-      uint32_t* mt = e->es.mt + (size_t)e->env * FE_MT_N;
-      int pos = e->es.mt_pos[e->env];
+      const int env = e->env, have = e->es.fix_have[env];
+      double* fp = e->es.fix_pose + (size_t)env * np * 7;
+      const unsigned fixed = e->es.fix_init[env] && have ? (1u << np) - 1u : (have ? (unsigned)e->es.fix_init_parts[env] : 0u);
+      uint32_t* mt = e->es.mt + (size_t)env * FE_MT_N;
+      int pos = e->es.mt_pos[env];
       const double half = 0.5 * (double)cfg->furn_rot_rand * 3.14159265358979323846 / 180.0;
       const double qx[4] = {cos(half), sin(half), 0.0, 0.0};
       const double r_xy = (double)cfg->furn_xyz_rand, r_rot = (double)cfg->furn_rot_rand;
       double px[FE_MAXPART], py[FE_MAXPART]; // placed so far, in double like the sampler's Qpos list
       for (int p = 0; p < np; ++p) {
+        const int qa = m->link_qadr[nrl + p];
+        if ((fixed >> p) & 1u) { // placed_objects_orig: at its remembered pose, z and quaternion included, no draw (:150-158)
+          px[p] = fp[7 * p]; py[p] = fp[7 * p + 1];
+          for (int k = 0; k < 7; ++k) w->qpos()[qa + k] = (float)fp[7 * p + k];
+        }
+      }
+      for (int p = 0; p < np; ++p) {
+        if ((fixed >> p) & 1u) continue;
+        const int qa = m->link_qadr[nrl + p];
         double x = 0, y = 0;
         for (int tries = 0; tries < 10000; ++tries) { // draw order of the reference: x, y per try; the rotation draw after a valid try
           x = ndadd((double)sc->part_init_pos[p][0], fe_mt_uniform(mt, &pos, -r_xy, r_xy));
           y = ndadd((double)sc->part_init_pos[p][1], fe_mt_uniform(mt, &pos, -r_xy, r_xy));
           bool valid = true;
-          for (int o = 0; o < p; ++o) {
+          for (int o = 0; o < np; ++o) { // the fixed parts and the parts placed before p; the outcome does not depend on the order
+            if (!(o < p || ((fixed >> o) & 1u)) || o == p) continue;
             const double dx = x - px[o], dy = y - py[o];
             if (ndsqrt(ndadd(ndmul(dx, dx), ndmul(dy, dy))) <= (double)sc->part_radius[o] + (double)sc->part_radius[p]) { valid = false; break; } // np.linalg.norm
           }
@@ -706,13 +740,17 @@ FE_FN void fe_env_reset_place(FeEnv* e) {
         }
         (void)fe_mt_uniform(mt, &pos, r_rot, r_rot); // sample_quat: rng.uniform(high=max, low=max), a draw whose value is always max
         px[p] = x; py[p] = y;
-        const int qa = m->link_qadr[nrl + p];
-        w->qpos()[qa] = (float)x; w->qpos()[qa + 1] = (float)y; w->qpos()[qa + 2] = sc->part_init_pos[p][2] + 0.01f;
+        const float z = sc->part_init_pos[p][2] + 0.01f;
+        w->qpos()[qa] = (float)x; w->qpos()[qa + 1] = (float)y; w->qpos()[qa + 2] = z;
         double q0[4] = {sc->part_init_quat[p][0], sc->part_init_quat[p][1], sc->part_init_quat[p][2], sc->part_init_quat[p][3]}, q[4];
         dq_mul(q, q0, qx);
         for (int k = 0; k < 4; ++k) w->qpos()[qa + 3 + k] = (float)q[k];
+        // init_pos.update: remembered as planted, so that a later fix_init start is this one bit for bit
+        fp[7 * p] = x; fp[7 * p + 1] = y; fp[7 * p + 2] = (double)z;
+        for (int k = 0; k < 4; ++k) fp[7 * p + 3 + k] = q[k];
       }
-      e->es.mt_pos[e->env] = pos;
+      e->es.fix_have[env] = 1;
+      e->es.mt_pos[env] = pos;
     }
   LANES_END
   fe_env_stabilise(e);
@@ -722,7 +760,6 @@ FE_FN void fe_env_reset_robot(FeEnv* e) {
   FeWarp* w = e->w;
   const fe_model* m = w->m;
   const fe_scene* sc = e->sc;
-  const fe_config* cfg = e->cfg;
   const int ng = m->ngeom;
   const int* rct = e->es.robot_contype + (size_t)e->env * ng;
   const int* rca = e->es.robot_conaff + (size_t)e->env * ng;
@@ -734,14 +771,7 @@ FE_FN void fe_env_reset_robot(FeEnv* e) {
         for (int i = lane; i < sc->ngrip; i += 32) w->qfrc_applied()[sc->grip_dof[i]] = w->bias()[sc->grip_dof[i]];
       }
       if (phase == 1) for (int g = lane; g < ng; g += 32) if (m->geom_tag[g] & FE_TAG_ROBOT) { w->contype()[g] = rct[g]; w->conaff()[g] = rca[g]; } // :1586-1595
-      if (lane == 0) { // _initialize_robot_pos (furniture.py:1761-1779): fresh noise on every call
-        uint32_t* mt = e->es.mt + (size_t)e->env * FE_MT_N;
-        int pos = e->es.mt_pos[e->env];
-        const double r = (double)cfg->agent_xyz_rand; // _init_random(shape, "agent") = rng.uniform(-r, r, size=7), furniture.py:336-349
-        for (int i = 0; i < sc->narm; ++i) w->qpos()[sc->arm_dof[i]] = (float)ndadd((double)sc->robot_init_qpos[i], fe_mt_uniform(mt, &pos, -r, r));
-        for (int i = 0; i < sc->ngrip; ++i) w->qpos()[sc->grip_dof[i]] = sc->robot_init_qpos[sc->narm + i];
-        e->es.mt_pos[e->env] = pos;
-      }
+      if (lane == 0) fe_init_robot_pos(e);
     LANES_END
     fe_fwd_step(e);
   }

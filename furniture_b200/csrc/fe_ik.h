@@ -159,6 +159,8 @@ FE_HDN void fe_ik_command(FeEnv* e, const FeIkArgs& ik, int arm_i, const float* 
   if (e->es.episode_len[e->env] == 0) {                     // _reset's tail: _initial_<arm>_hand_quat = _<arm>_hand_quat; controller.sync_state()
     for (int k = 0; k < 4; ++k) s_acc[k] = cur[k];
     v3cpy(target, hb);
+  } else if (e->es.arm_resync[e->env]) {                    // _connect sent the arm home: controller.sync_state() only (furniture.py:919-924)
+    v3cpy(target, hb);
   }
   // action[:3] * move_speed, axes swapped, clipped to the workspace (world position of the hand)
   const float mv[3] = {-a[1] * c->move_speed, a[0] * c->move_speed, a[2] * c->move_speed};
@@ -215,6 +217,7 @@ FE_FN void fe_env_ik_step_one(FeEnv* e, FeIkArgs ik, const float* action, float*
         fe_ik_command(e, ik, arm, a + arm * per);
         st->low[7 * na + arm] = na == 1 ? grip : a[na * per + arm];
       }
+      e->es.arm_resync[e->env] = 0;
     }
   LANES_END
   int fail = 0, reset_now = 0;

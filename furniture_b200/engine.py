@@ -221,7 +221,10 @@ def obs_columns(scene, robot_skip=0, robot_ob=True, object_ob=True, object_ob_al
 
 class Engine:
     def __init__(self, model: mjcf.Model, n_envs: int, device: int = 0, config: FeConfig | None = None, lib_path: str | None = None,
-                 dense: FeDenseConfig | None = None, ik=None, controller=None, obs_layout=None):
+                 dense: FeDenseConfig | None = None, ik=None, controller=None, obs_layout=None, fix_init=False, fix_init_parts=None,
+                 reset_robot_after_attach=None):
+        """`fix_init`, `fix_init_parts`, `reset_robot_after_attach`: the keys of config/furniture.py:116-127, :169-174 for every env of the
+        handle (set_reset_options changes them per env).  In a dense handle the dense reward's reset_robot_after_attach decides (None: follow it)."""
         path = lib_path or DEFAULT_LIB
         if not os.path.exists(path):
             raise RuntimeError(
@@ -271,6 +274,51 @@ class Engine:
         self.dense = dense
         if dense is not None:  # FurnitureSawyerDenseRewardEnv: the phase machine replaces the sparse reward inside fe_env_step
             self._chk(L.fe_enable_dense_reward(self.h, C.byref(dense)))
+        # _load_model (furniture.py:2013-2021): init_pos / init_quat start as the XML's *_initpos numerics, or None when it lists none
+        xml = mjcf.xml_init_poses(model.meta)
+        self._xml_listed = set(xml or ())
+        if xml is not None and self._xml_listed == set(self.em.part_names):
+            self.set("fix_pose", np.concatenate([xml[n] for n in self.em.part_names])[None, :])
+            self.set("fix_have", 1)
+        rra = reset_robot_after_attach
+        if dense is not None:  # fe_enable_dense_reward has set it from the dense reward's
+            if rra is not None and bool(rra) != bool(dense.reset_robot_after_attach):
+                raise ValueError("reset_robot_after_attach=%r disagrees with the dense reward's %r, which drives the phase machine and the arm"
+                                 % (rra, bool(dense.reset_robot_after_attach)))
+            rra = None
+        if fix_init or fix_init_parts or rra:
+            self.set_reset_options(fix_init=fix_init, fix_init_parts=fix_init_parts, reset_robot_after_attach=rra)
+
+    @staticmethod
+    def _part_names(parts):
+        return [n for n in (parts.split(",") if isinstance(parts, str) else list(parts or ())) if n]
+
+    def part_mask(self, parts):
+        """fix_init_parts (config/furniture.py:122-127: a set of part names, or the comma string str2set reads) -> bit mask over the parts in
+        XML order; an unknown name is a ValueError"""
+        names = self._part_names(parts)
+        unknown = sorted(set(names) - set(self.em.part_names))
+        if unknown:
+            raise ValueError("fix_init_parts names %s, which %s does not have (parts: %s)" % (unknown, self.model.meta.get("furniture"), list(self.em.part_names)))
+        return sum(1 << self.em.part_names.index(n) for n in set(names))
+
+    def set_reset_options(self, fix_init=None, fix_init_parts=None, reset_robot_after_attach=None, envs=None):
+        """fix_init (the furniture starts every episode where the env's first random placement, or the XML, put it: furniture.py:1519-1532),
+        fix_init_parts (only those parts do, the sampler places the others around them: :1389-1404) and reset_robot_after_attach (the arm goes
+        back to its start pose after every connection: :916-924), for the envs in `envs` (default: all); None leaves an option as it is.
+        They act from the env's next reset or connection on, inside the kernels."""
+        partial = self._xml_listed and self._xml_listed != set(self.em.part_names)
+        if partial and (fix_init or set(self._part_names(fix_init_parts)) - self._xml_listed):  # init_pos[body]: the reference's KeyError
+            raise ValueError("the XML of %s lists init poses for some parts only: fix_init, and fix_init_parts beyond %s, are undefined there"
+                             % (self.model.meta.get("furniture"), sorted(self._xml_listed)))
+        idx = np.arange(self.N) if envs is None else np.asarray(envs, dtype=np.int64).ravel()
+        for name, v in (("fix_init", fix_init), ("fix_init_parts", None if fix_init_parts is None else self.part_mask(fix_init_parts)),
+                        ("reset_robot_after_attach", reset_robot_after_attach)):
+            if v is None:
+                continue
+            cur = self.get(name)
+            cur[idx, 0] = int(v)
+            self.set(name, cur)
 
     def close(self):
         if getattr(self, "h", None) and self.h.value:
@@ -295,19 +343,24 @@ class Engine:
 
     _INT = {"order", "geom_contype", "geom_conaffinity", "eq_active", "touch", "flags", "ncon", "niter", "stats", "con_geom", "con_state", "group", "site_connected",
             "num_connected", "prev_num_connected", "touched", "picked", "episode_length", "done", "mt_pos", "preassembled", "num_connects",
-            "init_state", "init_pick", "init_mt_pos", "subtask_part"}
+            "init_state", "init_pick", "init_mt_pos", "subtask_part", "fix_init", "fix_init_parts", "fix_have", "reset_robot_after_attach"}
     _U32 = {"mt_state", "init_mt_state"}
+    _F64 = {"fix_pose"}
+
+    def _dtype(self, name, eb):
+        if eb == 8:
+            return np.float64 if name in self._F64 else np.uint64
+        return np.uint8 if eb == 1 else (np.uint32 if name in self._U32 else (np.int32 if name in self._INT else np.float32))
 
     def get(self, name):
         dim, eb = self.field_info(name)
-        dt = np.uint8 if eb == 1 else np.uint64 if eb == 8 else (np.uint32 if name in self._U32 else (np.int32 if name in self._INT else np.float32))
-        out = np.empty((self.N, dim), dtype=dt)
+        out = np.empty((self.N, dim), dtype=self._dtype(name, eb))
         self._chk(self.L.fe_get_field(self.h, name.encode(), out.ctypes.data_as(C.c_void_p), C.c_size_t(out.nbytes)))
         return out
 
     def set(self, name, value):
         dim, eb = self.field_info(name)
-        dt = np.uint8 if eb == 1 else np.uint64 if eb == 8 else (np.uint32 if name in self._U32 else (np.int32 if name in self._INT else np.float32))
+        dt = self._dtype(name, eb)
         v = np.ascontiguousarray(np.broadcast_to(np.asarray(value, dtype=dt), (self.N, dim)))
         self._chk(self.L.fe_set_field(self.h, name.encode(), v.ctypes.data_as(C.c_void_p), C.c_size_t(v.nbytes)))
 
@@ -448,6 +501,10 @@ class Engine:
         each of its resets an env in `envs` (default: all) keeps its start with probability 0.2 and otherwise picks one from the list
         uniformly, drawing from its own numpy RandomState(seed + 2**20 + env); the other envs do not pick.  [] or None ends the picking."""
         arrs = [self._state_arrays(st) for st in (states or [])]
+        partial = self._xml_listed and self._xml_listed != set(self.em.part_names)
+        if partial and (fix_init or set(self._part_names(fix_init_parts)) - self._xml_listed):  # init_pos[body]: the reference's KeyError
+            raise ValueError("the XML of %s lists init poses for some parts only: fix_init, and fix_init_parts beyond %s, are undefined there"
+                             % (self.model.meta.get("furniture"), sorted(self._xml_listed)))
         idx = np.arange(self.N) if envs is None else np.asarray(envs, dtype=np.int64).ravel()
         if idx.size and (idx.min() < 0 or idx.max() >= self.N):
             raise ValueError("envs must index the %d envs of this handle, got %s" % (self.N, idx.tolist()))

@@ -20,6 +20,7 @@ from . import mjcf
 from .dense import DENSE_DEFAULTS, DENSE_ENV_DEFAULTS, INFO_KEYS as DENSE_INFO_KEYS, dense_config
 from .engine import INFO_DIM, OBS_DEFAULTS, Engine, default_config, obs_columns
 
+RESET_DEFAULTS = dict(fix_init=False, fix_init_parts=None, reset_robot_after_attach=False)  # config/furniture.py:116-127, :169-174
 INFO_KEYS = ("num_connected", "episode_success", "episode_unstable", "episode_length", "ncon", "solver_iters")
 ENV_IDS = {"IKEASawyer-v0": "Sawyer", "FurnitureSawyerEnv": "Sawyer", "IKEABaxter-v0": "Baxter", "FurnitureBaxterEnv": "Baxter",
            "IKEASawyerDense-v0": "Sawyer", "furniture-sawyer-densereward-v0": "Sawyer", "FurnitureSawyerDenseRewardEnv": "Sawyer"}
@@ -52,8 +53,8 @@ def split_config(config):
     `furniture_name` wins over `furniture_id` as in furniture.py:157-161; keys the accelerated path has no use for (port, background,
     camera and rendering options ...) are returned so that callers can report them instead of failing on them.  `preassembled` (checked to be
     a recipe prefix), `num_connects`, `load_init_states`, `load_demo` and the observation flags `robot_ob`, `object_ob`, `object_ob_all`,
-    `subtask_ob` travel with the overrides when they are set (the flags when they differ from their defaults): they are keywords of the env
-    constructors."""
+    `subtask_ob` and the reset options `fix_init`, `fix_init_parts`, `reset_robot_after_attach` travel with the overrides when they are set
+    (the flags when they differ from their defaults): they are keywords of the env constructors."""
     from .engine import FeConfig
 
     cfg = dict(vars(config)) if hasattr(config, "__dict__") and not isinstance(config, dict) else dict(config or {})
@@ -69,7 +70,7 @@ def split_config(config):
     renamed = {"furn_xyz_rand": "furn_xyz_rand", "furn_rot_rand": "furn_rot_rand", "agent_xyz_rand": "agent_xyz_rand", "alignment_pos_dist": "alignment_pos_dist"}
     over = {renamed.get(k, k): v for k, v in cfg.items() if renamed.get(k, k) in fields and v is not None}
     ignored = sorted(k for k in cfg if k not in over and k not in ("furniture_name", "furniture_id", "control_type", "preassembled", "num_connects",
-                                                                   "load_init_states", "load_demo") + tuple(OBS_DEFAULTS))
+                                                                   "load_init_states", "load_demo") + tuple(OBS_DEFAULTS) + tuple(RESET_DEFAULTS))
     if prefix_length(cfg.get("preassembled")):
         over["preassembled"] = list(cfg["preassembled"])
     if cfg.get("num_connects") is not None:
@@ -80,6 +81,9 @@ def split_config(config):
     for k, default in OBS_DEFAULTS.items():  # furniture.py:103-107; a flag at its default changes nothing and is not passed on
         if cfg.get(k) is not None and bool(cfg[k]) != default:
             over[k] = bool(cfg[k])
+    for k in RESET_DEFAULTS:  # config/furniture.py:116-127, :169-174; False, None and the empty set are the defaults
+        if cfg.get(k):
+            over[k] = cfg[k] if k == "fix_init_parts" else bool(cfg[k])
     return name or "table_lack_0825", over, ignored
 
 
@@ -103,6 +107,7 @@ def split_dense_config(config):
     merged = dict(DENSE_ENV_DEFAULTS)
     merged.update({k: v for k, v in cfg.items() if v is not None})
     name, over, ignored = split_config(merged)
+    over.pop("reset_robot_after_attach", None)  # the dense reward's flag drives both its phase machine and the arm
     dense = {k: merged[k] for k in DENSE_DEFAULTS if k in merged}
     if "ctrl_penalty_coef" in over:
         dense["ctrl_penalty_coef"] = over["ctrl_penalty_coef"]
@@ -125,7 +130,7 @@ def apply_init_config(env, load_init_states=None, load_demo=None):
 class BatchedFurnitureEnv:
     def __init__(self, agent="Sawyer", furniture_name="table_lack_0825", num_envs=1, device=0, dense=None, control_type="impedance", ik=None,
                  preassembled=None, num_connects=None, load_init_states=None, load_demo=None, robot_ob=True, object_ob=True, object_ob_all=True,
-                 subtask_ob=False, **cfg_overrides):
+                 subtask_ob=False, fix_init=False, fix_init_parts=None, reset_robot_after_attach=None, **cfg_overrides):
         """`dense`: None for the sparse reward of FurnitureEnv; a dict of coefficient overrides (possibly empty) for the phase-based
         reward of FurnitureSawyerDenseRewardEnv, computed inside the step kernel (furniture_b200/dense.py).
         `control_type`: "impedance" (joint velocities, dof 9), "ik" (move 3, rotate 3, gripper, connect: dof 8) or "ik_quaternion" (the
@@ -140,7 +145,9 @@ class BatchedFurnitureEnv:
         starts from the list of `load_init_states` (see load_init_states), and every env starts from the first state of the demo `load_demo`.
         `robot_ob`, `object_ob`, `object_ob_all`, `subtask_ob`: the observation flags of config/furniture.py (furniture.py:103-107, :215-252,
         :1344-1387).  object_ob_all=False keeps in object_ob only the two parts of each env's current subtask (14 numbers, zeros when none is
-        left); subtask_ob=True adds their part ids + 1 (float32).  Each env's pair follows its connections and resets inside the kernels."""
+        left); subtask_ob=True adds their part ids + 1 (float32).  Each env's pair follows its connections and resets inside the kernels.
+        `fix_init`, `fix_init_parts`, `reset_robot_after_attach`: config/furniture.py:116-127, :169-174 (see set_reset_options).  A dense env
+        takes reset_robot_after_attach from `dense`, whose phase machine follows it (None: off, or the dense reward's)."""
         import torch
 
         if not torch.cuda.is_available():
@@ -180,7 +187,7 @@ class BatchedFurnitureEnv:
             raise NotImplementedError("control_type %r is not built" % control_type)
         self.obs_flags = dict(robot_ob=bool(robot_ob), object_ob=bool(object_ob), object_ob_all=bool(object_ob_all), subtask_ob=bool(subtask_ob))
         self.engine = Engine(self.model, num_envs, device=device, config=self.cfg, dense=self.dense_cfg, ik=self.ik_cfg, controller=self.ctl_cfg,
-                             obs_layout=self.obs_flags)
+                             obs_layout=self.obs_flags, fix_init=fix_init, fix_init_parts=fix_init_parts, reset_robot_after_attach=reset_robot_after_attach)
         self.num_envs = num_envs
         self.obs_dim, self.act_dim = self.engine.obs_dim, self.engine.act_dim
         self.n_objects = self.engine.scene.npart
@@ -218,6 +225,13 @@ class BatchedFurnitureEnv:
     def set_init_states(self, states):
         """the raw bank of recorded starts that the per-env fields init_state / init_pick index (Engine.set_init_states)"""
         self.engine.set_init_states(states)
+
+    def set_reset_options(self, fix_init=None, fix_init_parts=None, reset_robot_after_attach=None, envs=None):
+        """per env (`envs`, default: all; None leaves an option as it is): fix_init keeps the furniture's start the same in every episode (the
+        XML's init poses where it lists them, else the env's first random placement; no placement draw), fix_init_parts (a set or list of part
+        names, or a comma string) does so for those parts only and places the others around them, reset_robot_after_attach sends the arm back
+        to its start pose, with fresh noise, after every connection (furniture.py:916-924, :1389-1404, :1519-1532)"""
+        self.engine.set_reset_options(fix_init, fix_init_parts, reset_robot_after_attach, envs)
 
     def set_subtask(self, subtask, num_connects=None):
         """FurnitureEnv.set_subtask (furniture.py:204-207) with a scalar or an (N,) array each, so that the envs of one batch can train different
@@ -342,6 +356,8 @@ class MixedFurnitureEnv:
         counts = [envs_per_model] * len(self.names) if isinstance(envs_per_model, int) else list(envs_per_model)
         assert len(counts) == len(self.names)
         seed = cfg_overrides.pop("seed", 123)
+        if cfg_overrides.get("fix_init_parts"):
+            raise ValueError("fix_init_parts names the parts of one furniture model; set it per bucket with set_reset_options")
         self.buckets, self.offsets, off = [], [], 0
         for name, n in zip(self.names, counts):
             self.buckets.append(BatchedFurnitureEnv(agent, name, n, device=device, seed=seed + off, **cfg_overrides))

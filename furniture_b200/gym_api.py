@@ -33,7 +33,7 @@ class FurnitureGymB200:
         """`id`, `name` and the remaining keywords are what gym passes from the registration (env/__init__.py:19-114: id, name,
         furniture_name / furniture_id, background, port ...); options of the renderer are ignored, see env.split_config"""
         from .dense import dense_config
-        from .env import DENSE_IDS, NEW_CONTROLLERS, apply_init_config, control_options, prefix_length, split_config, split_dense_config
+        from .env import DENSE_IDS, NEW_CONTROLLERS, RESET_DEFAULTS, apply_init_config, control_options, prefix_length, split_config, split_dense_config
 
         if name not in AGENTS:
             raise ValueError("unknown env %s (this build accelerates %s)" % (name, sorted(AGENTS)))
@@ -48,6 +48,7 @@ class FurnitureGymB200:
         preassembled, num_connects = prefix_length(over.pop("preassembled", None)), over.pop("num_connects", None)
         load_init_states, load_demo = over.pop("load_init_states", None), over.pop("load_demo", None)
         self.obs_flags = dict(OBS_DEFAULTS, **{k: over.pop(k) for k in OBS_DEFAULTS if k in over})  # robot_ob ... subtask_ob (furniture.py:103-107)
+        reset_options = {k: over.pop(k) for k in RESET_DEFAULTS if k in over}  # fix_init, fix_init_parts, reset_robot_after_attach
         ctl = control_options(config)
         self.control_type, self.ik_cfg, self.ctl_cfg = ctl["control_type"], None, None
         agent = AGENTS[name]
@@ -68,7 +69,7 @@ class FurnitureGymB200:
 
             self.ik_cfg = ik_config(self.model, **dict(ctl["ik"], quaternion_mode=int(self.control_type == "ik_quaternion")))
         self.engine = Engine(self.model, 1, device=device, config=self.cfg, lib_path=lib_path, dense=self.dense_cfg, ik=self.ik_cfg, controller=self.ctl_cfg,
-                             obs_layout=self.obs_flags)
+                             obs_layout=self.obs_flags, **reset_options)
         self.n_objects = self.engine.scene.npart
         self._robot_skip = 0 if self.control_type == "impedance" else 14  # ik: robot_ob has no joint positions / velocities (furniture_sawyer.py:110-125)
         self._narms = max(1, int(self.engine.scene.narms))

@@ -178,6 +178,23 @@ BAXTER_BOTTOM_OFFSET = np.array([0.0, 0.0, -0.913])  # robots/baxter_robot.py:19
 GRIPPER_INIT_QPOS = np.array([0.020833, -0.020833])  # grippers/two_finger_gripper.py:22-23
 
 
+# the shipped furniture models whose XML carries no `<name>_initpos` numeric; every other one lists all its parts (none lists only some).  The
+# compiled scenes of compiled/ predate meta["xml_initpos_parts"], which compose_scene records, so this table stands in for it there
+NO_XML_INITPOS = frozenset(("bookcase_billy_0191", "bookcase_grevback_0484", "cabinet_akurum_0021", "chair_agam_0005", "table_hemnes_0539",
+                            "table_klubbo_0740", "table_liden_0921"))
+
+
+def xml_init_poses(meta):
+    """FurnitureEnv._load_model's init_pos / init_quat (furniture.py:2013-2021): part name -> the XML's (x, y, z, qw, qx, qy, qz) for the parts
+    the XML lists, or None for a model whose XML lists none (the reference's first reset then samples them)"""
+    listed = meta.get("xml_initpos_parts")
+    if listed is None:
+        listed = [] if meta.get("furniture") in NO_XML_INITPOS else list(meta["part_names"])
+    if not listed:
+        return None
+    return {n: np.asarray(meta["part_init_qpos"][n], dtype=np.float64)[:7] for n in listed}
+
+
 def place_unlisted_parts(part_names, listed, radii, seed):
     """Base placement of the parts whose XML carries no `<name>_initpos` numeric (7 of the shipped furniture models).
     Restates UniformRandomSampler.setup (models/tasks/placement_sampler.py:68-104 with the (0.7, 0.7, 0) table of
@@ -373,6 +390,7 @@ def compose_scene(agent="Sawyer", furniture="table_lack_0825", assets_root=None,
         import json
 
         meta["recipe_json"] = json.dumps(recipe)
+    meta["xml_initpos_parts"] = [n for n in part_names if n in init_qpos]
     init_qpos.update(place_unlisted_parts(part_names, init_qpos, radii, placement_seed))
     meta["part_init_qpos"] = init_qpos
     meta["part_radius"] = radii

@@ -103,7 +103,16 @@ int fe_sim_step(fe_handle* h, int nsub, void* stream);
    steps of the scene's assembly recipe before it places the robot, and the episode then succeeds at num_connects + preassembled connections,
    or with every part connected when num_connects is -1); init_state init_pick init_mt_state (624 x uint32) init_mt_pos (int32, one per env,
    read/write: the env's recorded start, see fe_set_init_states); subtask_part (2 x int32 per env, read only: _subtask_part1 / _subtask_part2,
-   the two parts of the env's current subtask, -1 / -1 when none is left -- see fe_set_obs_layout) */
+   the two parts of the env's current subtask, -1 / -1 when none is left -- see fe_set_obs_layout); fix_init fix_init_parts fix_have (int32,
+   one per env, read/write: config/furniture.py:116-127.  fix_init = 1 with fix_have = 1: the env's random-placement resets plant fix_pose and
+   draw nothing; otherwise they sample, planting the parts whose bit is set in fix_init_parts at fix_pose first when fix_have = 1, and store
+   the placement into fix_pose with fix_have = 1 -- furniture.py:1389-1404, :1519-1532; a recorded start ignores both); fix_pose (7 x float64
+   per part, XML order, read/write: position and quaternion w, x, y, z, the reference's init_pos / init_quat; fe_create leaves fix_have = 0,
+   the XML poses are the caller's to seed); reset_robot_after_attach (int32, one per env, read/write: every connection, the reset's
+   preassembly included, ends with _initialize_robot_pos, furniture.py:916-924, and the IK step re-seeds its position target; a dense handle
+   sets it from fe_dense_config.reset_robot_after_attach).  fe_set_field refuses flags outside {0, 1}, fix_init_parts bits at or beyond the
+   number of parts, non-finite fix_pose values or zero quaternions, fix_have = 1 for an env whose fix_pose was never written and, in a dense
+   handle, a reset_robot_after_attach that differs from the dense reward's */
 int fe_get_field(fe_handle* h, const char* name, void* dst_host, size_t bytes);
 int fe_set_field(fe_handle* h, const char* name, const void* src_host, size_t bytes);
 int fe_field_dim(fe_handle* h, const char* name, int* dim, int* elem_bytes);
