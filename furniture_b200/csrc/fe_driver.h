@@ -3,8 +3,8 @@
 #pragma once
 #include "fe_engine.h"
 
-#define FE_MAX_WPB 14      /* warps (= envs) per block of the sim / step / reset kernels */
-#define FE_EXTRA_BLOCKS 132 /* spare blocks of the step grid, one per SM of an H100 SXM: heavy envs get half-empty blocks */
+#define FE_MAX_WPB 16      /* warps (= envs) per block of the sim / step / reset kernels */
+#define FE_EXTRA_BLOCKS 132 /* spare blocks of the step grid, one per SM of an H100 SXM: heavy envs get partly empty blocks */
 
 struct FeState {
   int N;
@@ -17,6 +17,7 @@ struct FeState {
   int *flags, *ncon, *niter;                                            // [N]  flags: FE_FLAG_* bits
   int* order;                                                           // [N] rank -> env: the envs by the predicted work of their next step, heaviest first (written by fe_order_kernel)
   int* stats;                                                           // [N][FE_NSTAT] per call: the FE_STAT_* columns
+  float* coop;                                                          // [N][FeLayout::coop_words] the cooperative solver's arrays (FE_COOP_*)
 };
 
 // optional dump of one forward pass (all nullable, [N][dim])
@@ -32,6 +33,7 @@ FE_FN void fe_load(FeWarp* w, const FeState& s, int env) {
     LD(qpos, m->nq) LD(qvel, m->nv) LD(warm, m->nv) LD(ctrl, m->nu) LD(qfrc_applied, m->nr) LD(gravcomp, m->npart) LD(eq_data, 7 * m->neq) LD(mpos, 3 * m->nmov)
     LD(contype, m->ngeom) LD(conaff, m->ngeom) LD(eq_active, m->neq) LD(bias, m->nr)
     w->u()[lane] = 0; // FE_U_STAT + FE_NSTAT <= 32
+    if (lane == 0) w->coop = s.coop + (size_t)env * FE_LAY.coop_words;
   LANES_END
 #undef LD
 }

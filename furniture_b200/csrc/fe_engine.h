@@ -45,15 +45,20 @@ struct FeOpt {
 // table, no local-memory traffic to reach the slice.
 #define FE_SLICE_F(X) /* float arrays */ \
   X(qpos) X(qvel) X(warm) X(ctrl) X(qfrc_applied) X(gravcomp) X(eq_data) X(mpos) /* persistent state */ \
-  X(lpos) X(lquat) X(lmat) X(S) X(lvel) X(lacc) X(lfrc) X(linert) X(lcrb) X(Mr) X(Lr) X(fs) X(as) X(bias) X(lacc2) /* kinematics / dynamics */ \
+  X(lpos) X(lquat) X(lmat) X(S) X(lvel) X(lacc) X(lfrc) X(linert) X(lcrb) X(Mr) X(fs) X(as) X(bias) X(lacc2) /* kinematics / dynamics */ \
   X(gpos) X(gmat) /* collision */ \
-  X(c_dist) X(c_pos) X(c_frame) X(c_aref) X(c_D) X(c_mu) X(c_fric) X(c_jar) X(c_jv) X(c_f) /* contacts (SoA, maxcon each) */ \
+  X(c_dist) X(c_pos) X(c_frame) X(c_aref) X(c_D) X(c_mu) X(c_fric) X(c_jar) X(c_f) /* contacts (SoA, maxcon each) */ \
   X(w_r1) X(w_G) X(w_aref) X(w_D) X(w_jar) X(w_jv) X(w_f) /* welds (neq each) */ \
-  X(l_sign) X(l_aref) X(l_D) X(l_jar) X(l_jv) X(l_f) /* joint limits (nr each) */ \
-  X(x) X(Ma) X(grad) X(search) X(Mv) X(fc) X(H) X(Jc) X(scr) /* solver */
+  X(l_sign) X(l_aref) X(l_D) X(l_jar) X(l_f) /* joint limits (nr each) */ \
+  X(x) X(grad) X(search) X(Mv) X(fc) X(Hm) X(Jc) X(scr) /* solver */
 #define FE_SLICE_I(X) /* int arrays */ \
-  X(contype) X(conaff) X(eq_active) X(cand) X(touch) X(c_geom) X(c_link) X(c_state) X(c_kind) X(plist) X(first) X(iscr) X(colmap) X(skip) \
+  X(contype) X(conaff) X(eq_active) X(cand) X(touch) X(c_geom) X(c_link) X(c_state) X(c_kind) X(plist) X(first) X(iscr) X(colmap) \
   X(u) /* uniform scalars: the FE_U_* words */
+// Arrays only the cooperative fallback solver (fe_solve_coop) uses: the full tri(nv) Hessian, its line-search rows and block
+// flags.  They live in a per-env block of global memory (FeState::coop, reached through FeWarp::coop), not in the slice: the
+// fallback runs only for a component beyond 32 dofs or 32 contacts, and keeping them out of the slice lets more envs share an SM.
+#define FE_COOP_F(X) X(H) X(Ma) X(c_jv) X(l_jv)
+#define FE_COOP_I(X) X(skip)
 
 #define FE_NSTAT 28 /* per-call statistics: the FE_STAT_* columns of the `stats` field (include/furniture_b200.h) */
 // words of u: the per-call scalars, then the statistics (column c of `stats` in word FE_U_STAT + c)
@@ -61,8 +66,9 @@ enum { FE_U_NCON = 0, FE_U_NCAND = 1, FE_U_FLAGS = 2, FE_U_NITER = 3, FE_U_STAT 
 static_assert(FE_STAT_NEWTON_LS < FE_NSTAT && FE_U_STAT + FE_NSTAT <= 32, "u holds every column and is cleared by one lane each");
 struct FeLayout {
 #define X(f) int f;
-  FE_SLICE_F(X) FE_SLICE_I(X)
+  FE_SLICE_F(X) FE_SLICE_I(X) FE_COOP_F(X) FE_COOP_I(X)
 #undef X
+  int coop_words; // size of an env's block of FE_COOP_* arrays
 };
 static FeLayout fe_h_lay; // host copy: what the lane-emulated build reads, and what the CUDA build uploads
 #if FE_DEVICE_BUILD
@@ -78,10 +84,11 @@ __constant__ FeLayout fe_c_lay;
 #define FE_LAY fe_h_lay
 #endif
 
-#define FE_WARP_HDR_WORDS 10 /* sizeof(FeWarp) is 6 words; the 4 spare words keep every array at the offset the kernels were tuned with */
+#define FE_WARP_HDR_WORDS 10 /* sizeof(FeWarp) is 8 words; the 2 spare words keep every array at the offset the kernels were tuned with */
 struct FeWarp { // header at word 0 of the slice
   const fe_model* m;
   FeOpt opt;
+  float* coop; // this env's block of the FE_COOP_* arrays in global memory (set by fe_load)
   // Device: the slice address is rebuilt from the dynamic shared-memory symbol plus the warp's byte offset, so that the compiler
   // sees a shared-memory pointer and emits LDS / STS with 32-bit addresses (through the generic `this` every slice access was
   // a generic LD.E / ST.E with a 64-bit address pair).
@@ -96,6 +103,12 @@ struct FeWarp { // header at word 0 of the slice
 #define X(f) FE_ACC int* f() const { return (int*)base_() + FE_LAY.f; }
   FE_SLICE_I(X)
 #undef X
+#define X(f) FE_ACC float* f() const { return coop + FE_LAY.f; }
+  FE_COOP_F(X)
+#undef X
+#define X(f) FE_ACC int* f() const { return (int*)coop + FE_LAY.f; }
+  FE_COOP_I(X)
+#undef X
 };
 static_assert(sizeof(FeWarp) <= 4 * FE_WARP_HDR_WORDS, "slice header too small");
 
@@ -108,21 +121,29 @@ FE_BOTH int fe_layout_build(FeLayout* L, const fe_model* m, const FeOpt& opt) {
 #define CARVE(field, n) L->field = o; o += (n);
   CARVE(qpos, nq) CARVE(qvel, nv) CARVE(warm, nv) CARVE(ctrl, nu) CARVE(qfrc_applied, nr) CARVE(gravcomp, np) CARVE(eq_data, 7 * ne) CARVE(mpos, 3 * m->nmov)
   CARVE(contype, ng) CARVE(conaff, ng) CARVE(eq_active, ne)
-  CARVE(lpos, 3 * nl) CARVE(lquat, 4 * nl) CARVE(lmat, 9 * nl) CARVE(S, 6 * nr) CARVE(lvel, 6 * nl) CARVE(lacc, 6 * nl) CARVE(lfrc, 6 * nl)
+  CARVE(lpos, 3 * nl) CARVE(lquat, 4 * nl) CARVE(lmat, 9 * nl) CARVE(S, 6 * nr) CARVE(lvel, 6 * nl) CARVE(lfrc, 6 * nl)
   L->lacc2 = L->lfrc; /* RNE wrench (smooth stage) and solver link accelerations are never live together */
-  CARVE(linert, 10 * nl) CARVE(lcrb, (10 * nr > 96 ? 10 * nr : 96)) CARVE(Mr, nr * nr) CARVE(Lr, fe_tri(nr)) CARVE(fs, nv) CARVE(as, nv) CARVE(bias, nr)
+  CARVE(linert, 10 * nl) CARVE(lcrb, (10 * nr > 96 ? 10 * nr : 96)) CARVE(Mr, nr * nr) CARVE(fs, nv) CARVE(as, nv) CARVE(bias, nr)
   CARVE(touch, np)
   CARVE(c_dist, mc) CARVE(c_pos, 3 * mc) CARVE(c_frame, 6 * mc) CARVE(c_aref, 3 * mc) CARVE(c_D, 2 * mc) CARVE(c_mu, mc) CARVE(c_fric, mc)
-  CARVE(c_jar, 3 * mc) CARVE(c_jv, 3 * mc) CARVE(c_f, 3 * mc) CARVE(c_geom, mc) CARVE(c_link, mc) CARVE(c_state, mc) CARVE(c_kind, mc) CARVE(plist, 9 * np)
+  CARVE(c_jar, 3 * mc) CARVE(c_f, 3 * mc) CARVE(c_geom, mc) CARVE(c_link, mc) CARVE(c_state, mc) CARVE(c_kind, mc) CARVE(plist, 9 * np)
   CARVE(w_r1, 3 * ne) CARVE(w_G, 9 * ne) CARVE(w_aref, 6 * ne) CARVE(w_D, 6 * ne) CARVE(w_jar, 6 * ne) CARVE(w_jv, 6 * ne) CARVE(w_f, 6 * ne)
-  CARVE(l_sign, nr) CARVE(l_aref, nr) CARVE(l_D, nr) CARVE(l_jar, nr) CARVE(l_jv, nr) CARVE(l_f, nr)
-  CARVE(x, nv) CARVE(Ma, nv) CARVE(grad, nv) CARVE(search, nv) CARVE(Mv, nv) CARVE(fc, nv)
+  CARVE(l_sign, nr) CARVE(l_aref, nr) CARVE(l_D, nr) CARVE(l_jar, nr) CARVE(l_f, nr)
+  CARVE(x, nv) CARVE(grad, nv) CARVE(search, nv) CARVE(Mv, nv) CARVE(fc, nv)
   L->Jc = L->lcrb; /* composite inertias (smooth stage) vs row staging of fe_build_H */
-  CARVE(scr, 2 * 32) CARVE(first, nv) CARVE(skip, nv) CARVE(iscr, 32) CARVE(colmap, 32) CARVE(u, FE_U_STAT + FE_NSTAT)
-  // H (solver) and the collision scratch (geom poses, candidate list) are never live together: overlay them
-  const int hwords = fe_tri(nv), cwords = 12 * ng + FE_CAND_WORDS;
-  L->H = o; L->gpos = o; L->gmat = o + 3 * ng; L->cand = o + 12 * ng;
-  o += hwords > cwords ? hwords : cwords;
+  CARVE(scr, 2 * 32) CARVE(first, nv) CARVE(iscr, 32) CARVE(colmap, 32) CARVE(u, FE_U_STAT + FE_NSTAT)
+  // Three users of one region, never live together: the RNE link accelerations (smooth stage), the collision scratch (geom
+  // poses, candidate list) and the constant part of the register solver's Hessian (fe_solve_comp: packed lower triangle over
+  // the component's at most 32 active dofs).
+  const int nh = nv < 32 ? nv : 32, hwords = fe_tri(nh), cwords = 12 * ng + FE_CAND_WORDS, awords = 6 * nl;
+  L->Hm = o; L->gpos = o; L->gmat = o + 3 * ng; L->cand = o + 12 * ng; L->lacc = o;
+  o += hwords > cwords ? (hwords > awords ? hwords : awords) : (cwords > awords ? cwords : awords);
+  // the cooperative solver's arrays, in the env's block of global memory
+  int g = 0;
+#define GCARVE(field, n) L->field = g; g += (n);
+  GCARVE(H, fe_tri(nv)) GCARVE(Ma, nv) GCARVE(c_jv, 3 * mc) GCARVE(l_jv, nr) GCARVE(skip, nv)
+#undef GCARVE
+  L->coop_words = g;
 #undef CARVE
   return o;
 }
@@ -2066,7 +2087,7 @@ FE_HD void fe_solve_free_parts(FeWarp* w, unsigned skipmask) {
 // free parts that only touch the static world (8 lanes per part, fe_solve_parts_grouped), the robot block when its only
 // rows are joint limits (fe_solve_robot_limits), and the coupled component -- robot block with contacts, parts in contact
 // with the robot or each other, welded parts -- solved by fe_solve_comp with its rows in registers.  A component beyond 32
-// dofs or 32 contacts falls back to the cooperative shared-memory solver over all dofs (fe_solve_coop).
+// dofs or 32 contacts falls back to the cooperative solver over all dofs (fe_solve_coop; its Hessian in global memory).
 FE_FN void fe_solve(FeWarp* w) {
   const fe_model* m = w->m;
   const int ncon = w->u()[FE_U_NCON], ne = m->neq, np = m->npart, nrl = m->nrlink, nr = m->nr;
@@ -2140,7 +2161,7 @@ FE_FN void fe_solve(FeWarp* w) {
     FE_TICK(w->u() + FE_U_STAT, FE_STAT_SOLVE_COMP)
     return;
   }
-  fe_solve_coop(w, cplmask); // fallback: the cooperative solver in shared memory, over all dofs
+  fe_solve_coop(w, cplmask); // fallback: the cooperative solver over all dofs (FE_COOP_* arrays in global memory)
 }
 
 // ---------------------------------------------------------------- mj_Euler + mj_advance

@@ -61,8 +61,8 @@ extern "C" __global__ void __launch_bounds__(32 * FE_MAX_WPB) fe_env_reset_kerne
 // the big Newton solve) bound the whole step by their own latency, which is lowest when few warps share the SM: they get
 // blocks with only `heavy_k` of the warp slots used, launched first, while the light envs fill the other SMs.
 #define FE_ORDER_BUCKETS 256
-#define FE_ORDER_HEAVY_SHIFT 18 /* heavy: 18 buckets above the median, 2^(18/16) = 2.2x the median work */
-#define FE_ORDER_HEAVY_K 7      /* warp slots used in a block of heavy envs (7 of 14); half the block where it holds fewer than 8 */
+#define FE_ORDER_HEAVY_SHIFT 24 /* heavy: 24 buckets above the median, 2^(24/16) = 2.8x the median work */
+#define FE_ORDER_HEAVY_K 3      /* warp slots used in a block of heavy envs (3 of 16); half the block where it holds fewer than 4 */
 #define FE_ORDER_DECAY 0.85f    /* per-step decay of an env's predicted work */
 extern "C" __global__ void __launch_bounds__(1024) fe_order_kernel(int N, const int* __restrict__ stats, int* __restrict__ order, int* __restrict__ slots, int nslots,
                                                         int wpb, float* __restrict__ pred) {

@@ -21,6 +21,14 @@
 // 6x6 matrix K per pair of links in contact (as in fe_newton_regs), factored and solved in registers by FE_REG_CHOL_SOLVE.
 #pragma once
 
+FE_BOTH int fe_popc(unsigned v) {
+#if defined(__CUDA_ARCH__)
+  return __popc(v);
+#else
+  return __builtin_popcount(v);
+#endif
+}
+
 template <int NMAX>
 FE_FN void fe_solve_comp(FeWarp* w, int nA, int ncc, unsigned cplmask, int robot_in) {
   const fe_model* m = w->m;
@@ -31,8 +39,10 @@ FE_FN void fe_solve_comp(FeWarp* w, int nA, int ncc, unsigned cplmask, int robot
   int* const ccl = (int*)w->Jc(); // [32] component contacts (set by the caller)
   int* const lidx = ccl + 32;     // [64] per-link contact lists: contact | side << 8 (side 1 = the link is the B side)
   int* const lptr = w->first();   // [nlink + 1]
-  float* const Hm = w->H();       // packed lower triangle in solver coordinates: M + weld terms (constant during the solve)
+  float* const Hm = w->Hm();      // packed lower triangle over the active dofs (row i = colmap[i]): M + weld terms (constant during the solve)
 #define COMP_INLINK(l) ((l) < nrl ? robot_in : (int)((cplmask >> ((l) - nrl)) & 1u))
+  // position of active dof z in colmap: robot dofs first, then the coupled parts in order
+#define COMP_POS(z) ((z) < nr ? (z) : (robot_in ? nr : 0) + 6 * fe_popc(cplmask & ((1u << (((z) - nr) / 6)) - 1u)) + ((z) - nr) % 6)
 
   FE_PRIV(int, z_); FE_PRIV(float, x_); FE_PRIV(float, as_); FE_PRIV(float, r_); FE_PRIV(float, fc_); FE_PRIV(float, s_); FE_PRIV(float, Ms_);
   FE_PRIV(float, lsg_); FE_PRIV(float, lar_); FE_PRIV(float, lD_); FE_PRIV(int, sub_);
@@ -50,7 +60,7 @@ FE_FN void fe_solve_comp(FeWarp* w, int nA, int ncc, unsigned cplmask, int robot
     // rows of the coupled parts start with zeros left of their own block (M is block diagonal; weld terms are added below)
     for (int p = 0; p < np; ++p)
       if ((cplmask >> p) & 1u) {
-        const int z = nr + 6 * p;
+        const int z = COMP_POS(nr + 6 * p);
         for (int j = lane; j < z; j += 32)
 #pragma unroll
           for (int i = 0; i < 6; ++i) Hm[fe_tri(z + i) + j] = 0.f;
@@ -87,7 +97,7 @@ FE_FN void fe_solve_comp(FeWarp* w, int nA, int ncc, unsigned cplmask, int robot
         for (int j = 0; j <= d; ++j) Hm[fe_tri(d) + j] = w->Mr()[d * nr + j];
     for (int p = lane; p < np; p += 32)
       if ((cplmask >> p) & 1u) {
-        const int z = nr + 6 * p;
+        const int z = COMP_POS(nr + 6 * p);
         float A[21];
         fe_inert_sym6(A, w->linert() + 10 * (nrl + p), 0.f);
 #pragma unroll
@@ -124,7 +134,7 @@ FE_FN void fe_solve_comp(FeWarp* w, int nA, int ncc, unsigned cplmask, int robot
               for (int k = 0; k < 3; ++k) col[k] = sg * w->w_G()[9 * e + 3 * k + jj];
             }
             w->scr()[j] = col[0]; w->scr()[16 + j] = col[1]; w->scr()[32 + j] = col[2];
-            w->iscr()[j] = nr + 6 * ((sideA ? A : B) - nrl) + jj;
+            w->iscr()[j] = COMP_POS(nr + 6 * ((sideA ? A : B) - nrl) + jj);
           }
         LANES_END
         LANES_BEGIN
@@ -360,11 +370,11 @@ FE_FN void fe_solve_comp(FeWarp* w, int nA, int ncc, unsigned cplmask, int robot
     // ---- Newton direction: H rows in registers
     REGS_BEGIN
       const int i = lane, zi = PV(z_);
-      const float* Hi = Hm + fe_tri(zi >= 0 ? zi : 0);
+      const float* Hi = Hm + fe_tri(zi >= 0 ? i : 0);
 #pragma unroll
       for (int j = 0; j < NMAX; ++j) {
         float v = (j == i) ? 1.f : 0.f;
-        if (j <= i && i < nA) v = Hi[w->colmap()[j]];
+        if (j <= i && i < nA) v = Hi[j];
         PV(row_)[j] = v;
       }
       if (PV(lsg_) != 0.f && PV(lsg_) * PV(x_) - PV(lar_) < 0.f) { // active joint-limit row: D on the diagonal
@@ -488,4 +498,5 @@ FE_FN void fe_solve_comp(FeWarp* w, int nA, int ncc, unsigned cplmask, int robot
 #undef COMP_MULM
 #undef COMP_COST
 #undef COMP_INLINK
+#undef COMP_POS
 }
