@@ -414,6 +414,15 @@ class Engine:
         self.obs_dim = self.scene.obs_dim = int(self.L.fe_obs_dim(self.h))
         self.scene.obs_layout = (0 if robot_ob else 1) | (0 if object_ob else 2) | (0 if object_ob_all else 4) | (8 if subtask_ob else 0)
 
+    def obs_columns(self):
+        """(key -> columns of a device row, key -> width) of the obs dict under this handle's flags (the module's obs_columns); the widths of
+        object_ob, subtask_ob, robot_ob and phase_ob are 0 where the dict has no such entry.  Under the IK and controller control types robot_ob
+        drops each arm's 14 joint positions and velocities (furniture_sawyer.py:110-125, furniture_baxter.py:137-160)."""
+        skip = 0 if self.ik is None and self.controller is None else 14
+        cols = obs_columns(self.scene, skip, **self.obs_flags)
+        widths = {k: len(np.arange(self.obs_dim)[cols[k]]) if k in cols else 0 for k in ("object_ob", "subtask_ob", "robot_ob", "phase_ob")}
+        return cols, widths
+
     def set_max_episode_steps(self, n):
         self._chk(self.L.fe_set_max_episode_steps(self.h, int(n)))
         self.cfg.max_episode_steps = int(n)
@@ -501,10 +510,6 @@ class Engine:
         each of its resets an env in `envs` (default: all) keeps its start with probability 0.2 and otherwise picks one from the list
         uniformly, drawing from its own numpy RandomState(seed + 2**20 + env); the other envs do not pick.  [] or None ends the picking."""
         arrs = [self._state_arrays(st) for st in (states or [])]
-        partial = self._xml_listed and self._xml_listed != set(self.em.part_names)
-        if partial and (fix_init or set(self._part_names(fix_init_parts)) - self._xml_listed):  # init_pos[body]: the reference's KeyError
-            raise ValueError("the XML of %s lists init poses for some parts only: fix_init, and fix_init_parts beyond %s, are undefined there"
-                             % (self.model.meta.get("furniture"), sorted(self._xml_listed)))
         idx = np.arange(self.N) if envs is None else np.asarray(envs, dtype=np.int64).ravel()
         if idx.size and (idx.min() < 0 or idx.max() >= self.N):
             raise ValueError("envs must index the %d envs of this handle, got %s" % (self.N, idx.tolist()))

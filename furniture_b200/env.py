@@ -18,14 +18,15 @@ import numpy as np
 
 from . import mjcf
 from .dense import DENSE_DEFAULTS, DENSE_ENV_DEFAULTS, INFO_KEYS as DENSE_INFO_KEYS, dense_config
-from .engine import INFO_DIM, OBS_DEFAULTS, Engine, default_config, obs_columns
+from .engine import INFO_DIM, OBS_DEFAULTS, Engine, default_config
 
 RESET_DEFAULTS = dict(fix_init=False, fix_init_parts=None, reset_robot_after_attach=False)  # config/furniture.py:116-127, :169-174
 INFO_KEYS = ("num_connected", "episode_success", "episode_unstable", "episode_length", "ncon", "solver_iters")
-ENV_IDS = {"IKEASawyer-v0": "Sawyer", "FurnitureSawyerEnv": "Sawyer", "IKEABaxter-v0": "Baxter", "FurnitureBaxterEnv": "Baxter",
-           "IKEASawyerDense-v0": "Sawyer", "furniture-sawyer-densereward-v0": "Sawyer", "FurnitureSawyerDenseRewardEnv": "Sawyer"}
+# env id or class name (env/__init__.py:19-114) -> (agent, whether it is FurnitureSawyerDenseRewardEnv, env/__init__.py:103-114)
+ENV_IDS = {"IKEASawyer-v0": ("Sawyer", False), "FurnitureSawyerEnv": ("Sawyer", False), "IKEABaxter-v0": ("Baxter", False),
+           "FurnitureBaxterEnv": ("Baxter", False), "IKEASawyerDense-v0": ("Sawyer", True), "furniture-sawyer-densereward-v0": ("Sawyer", True),
+           "FurnitureSawyerDenseRewardEnv": ("Sawyer", True)}
 NEW_CONTROLLERS = ("position", "position_orientation", "joint_impedance", "joint_torque", "joint_velocity")  # furniture.py:41-47
-DENSE_IDS = {"IKEASawyerDense-v0", "furniture-sawyer-densereward-v0", "FurnitureSawyerDenseRewardEnv"}  # env/__init__.py:103-114
 # furniture_id -> name: the reference numbers the sorted objects/*.xml (furniture/env/models/__init__.py:11-19)
 FURNITURE_NAMES = (
     "bed_dalselv_0270 bench_bjoderna_0208 bench_bjursta_0210 block bookcase_agerum_0006 bookcase_besta_0165 bookcase_besta_0170 bookcase_besta_0172 "
@@ -51,10 +52,10 @@ def prefix_length(preassembled):
 def split_config(config):
     """Reference-style config (argparse Namespace or dict, config/furniture.py) -> (furniture name, FeConfig overrides, ignored keys).
     `furniture_name` wins over `furniture_id` as in furniture.py:157-161; keys the accelerated path has no use for (port, background,
-    camera and rendering options ...) are returned so that callers can report them instead of failing on them.  `preassembled` (checked to be
-    a recipe prefix), `num_connects`, `load_init_states`, `load_demo` and the observation flags `robot_ob`, `object_ob`, `object_ob_all`,
-    `subtask_ob` and the reset options `fix_init`, `fix_init_parts`, `reset_robot_after_attach` travel with the overrides when they are set
-    (the flags when they differ from their defaults): they are keywords of the env constructors."""
+    camera and rendering options, the speeds where no control type reads them ...) are returned so that callers can report them instead of
+    failing on them.  `preassembled` (checked to be a recipe prefix), `num_connects`, `load_init_states`, `load_demo` and the observation flags
+    `robot_ob`, `object_ob`, `object_ob_all`, `subtask_ob` and the reset options `fix_init`, `fix_init_parts`, `reset_robot_after_attach` travel
+    with the overrides when they are set (the flags when they differ from their defaults): they are keywords of build_engine."""
     from .engine import FeConfig
 
     cfg = dict(vars(config)) if hasattr(config, "__dict__") and not isinstance(config, dict) else dict(config or {})
@@ -71,6 +72,8 @@ def split_config(config):
     over = {renamed.get(k, k): v for k, v in cfg.items() if renamed.get(k, k) in fields and v is not None}
     ignored = sorted(k for k in cfg if k not in over and k not in ("furniture_name", "furniture_id", "control_type", "preassembled", "num_connects",
                                                                    "load_init_states", "load_demo") + tuple(OBS_DEFAULTS) + tuple(RESET_DEFAULTS))
+    if "ik" in control_options(cfg):  # the speeds reach the IK or the controller
+        ignored = [k for k in ignored if k not in ("move_speed", "rotate_speed")]
     if prefix_length(cfg.get("preassembled")):
         over["preassembled"] = list(cfg["preassembled"])
     if cfg.get("num_connects") is not None:
@@ -127,11 +130,21 @@ def apply_init_config(env, load_init_states=None, load_demo=None):
         env.load_init_states(states(load_init_states))
 
 
-class BatchedFurnitureEnv:
-    def __init__(self, agent="Sawyer", furniture_name="table_lack_0825", num_envs=1, device=0, dense=None, control_type="impedance", ik=None,
-                 preassembled=None, num_connects=None, load_init_states=None, load_demo=None, robot_ob=True, object_ob=True, object_ob_all=True,
-                 subtask_ob=False, fix_init=False, fix_init_parts=None, reset_robot_after_attach=None, **cfg_overrides):
-        """`dense`: None for the sparse reward of FurnitureEnv; a dict of coefficient overrides (possibly empty) for the phase-based
+def env_options(config, dense_reward=False):
+    """Reference-style config of the sparse env, or of the dense-reward env -> (furniture name, keywords of build_engine, ignored keys)"""
+    if dense_reward:
+        furniture, over, dense, ignored = split_dense_config(config)
+        over["dense"] = dense
+    else:
+        furniture, over, ignored = split_config(config)
+    return furniture, dict(over, **control_options(config)), ignored
+
+
+def build_engine(agent, furniture_name, num_envs, device=0, lib_path=None, dense=None, control_type="impedance", ik=None, preassembled=None,
+                 num_connects=None, load_init_states=None, load_demo=None, robot_ob=True, object_ob=True, object_ob_all=True, subtask_ob=False,
+                 fix_init=False, fix_init_parts=None, reset_robot_after_attach=None, **cfg_overrides):
+    """The Engine of `num_envs` envs of `agent` + `furniture_name` that both env surfaces run; `lib_path` as for Engine.  The keywords:
+        `dense`: None for the sparse reward of FurnitureEnv; a dict of coefficient overrides (possibly empty) for the phase-based
         reward of FurnitureSawyerDenseRewardEnv, computed inside the step kernel (furniture_b200/dense.py).
         `control_type`: "impedance" (joint velocities, dof 9), "ik" (move 3, rotate 3, gripper, connect: dof 8) or "ik_quaternion" (the
         rotation as a quaternion relative to the hand: dof 9); the inverse kinematics and its three closed-loop repeats run inside the
@@ -147,7 +160,50 @@ class BatchedFurnitureEnv:
         :1344-1387).  object_ob_all=False keeps in object_ob only the two parts of each env's current subtask (14 numbers, zeros when none is
         left); subtask_ob=True adds their part ids + 1 (float32).  Each env's pair follows its connections and resets inside the kernels.
         `fix_init`, `fix_init_parts`, `reset_robot_after_attach`: config/furniture.py:116-127, :169-174 (see set_reset_options).  A dense env
-        takes reset_robot_after_attach from `dense`, whose phase machine follows it (None: off, or the dense reward's)."""
+        takes reset_robot_after_attach from `dense`, whose phase machine follows it (None: off, or the dense reward's).
+    The other keywords override FeConfig fields (default_config).  The engine records `control_type` and `resize_factor`."""
+    cfg = default_config(**cfg_overrides)
+    # furn_size_rand (config/furniture.py:196-201): the reference draws one size factor per env process while loading the model.
+    # A handle shares one model: the batch takes env 0's factor (the first draw of RandomState(seed)); every env's generator
+    # still spends its draws like the reference's.  Different sizes side by side = several handles (MixedFurnitureEnv).
+    resize_factor = None
+    if cfg.furn_size_rand != 0:
+        r = float(cfg.furn_size_rand)
+        resize_factor = 1 + float(np.random.RandomState(int(cfg.seed)).uniform(-r, r, 1)[0])
+    if control_type in NEW_CONTROLLERS:
+        if agent != "Sawyer":
+            raise NotImplementedError("the torque controllers are built for the Sawyer env")
+        agent = "SawyerTorque"  # robots/sawyer/robot_torque.xml (furniture.py:1893-1899)
+    elif control_type in ("ik", "ik_quaternion"):
+        if agent not in ("Sawyer", "Baxter"):
+            raise NotImplementedError("control_type='%s' is built for the Sawyer and Baxter envs" % control_type)
+    elif control_type != "impedance":
+        raise NotImplementedError("control_type %r is not built" % control_type)
+    model = mjcf.load_scene(agent, furniture_name, resize_factor=resize_factor)
+    ik_cfg = ctl_cfg = None
+    if control_type in ("ik", "ik_quaternion"):
+        from .ik import ik_config
+
+        ik_cfg = ik_config(model, **dict(ik or {}, quaternion_mode=int(control_type == "ik_quaternion")))
+    elif control_type in NEW_CONTROLLERS:
+        from .controllers import ctl_config
+
+        ctl_cfg = ctl_config(control_type, model=model, move_speed=(ik or {}).get("move_speed", 0.1))
+    obs_flags = dict(robot_ob=bool(robot_ob), object_ob=bool(object_ob), object_ob_all=bool(object_ob_all), subtask_ob=bool(subtask_ob))
+    engine = Engine(model, num_envs, device=device, config=cfg, lib_path=lib_path, dense=dense_config(**dense) if dense is not None else None,
+                    ik=ik_cfg, controller=ctl_cfg, obs_layout=obs_flags, fix_init=fix_init, fix_init_parts=fix_init_parts,
+                    reset_robot_after_attach=reset_robot_after_attach)
+    engine.control_type, engine.resize_factor = control_type, resize_factor
+    if prefix_length(preassembled) or num_connects is not None:
+        engine.set_subtask(prefix_length(preassembled), num_connects)
+    apply_init_config(engine, load_init_states, load_demo)
+    return engine
+
+
+class BatchedFurnitureEnv:
+    def __init__(self, agent="Sawyer", furniture_name="table_lack_0825", num_envs=1, device=0, **options):
+        """`num_envs` envs on CUDA device `device`; `options` are the keywords of build_engine (reward, control type, starts, observation
+        flags, reset options, FeConfig overrides)."""
         import torch
 
         if not torch.cuda.is_available():
@@ -156,59 +212,18 @@ class BatchedFurnitureEnv:
         self.device = torch.device("cuda", device)
         torch.cuda.set_device(self.device)
         torch.zeros(1, device=self.device)  # make sure the primary context exists before the library binds to it
-        self.cfg = default_config(**cfg_overrides)
-        # furn_size_rand (config/furniture.py:196-201): the reference draws one size factor per env process while loading the model.
-        # A handle shares one model: the batch takes env 0's factor (the first draw of RandomState(seed)); every env's generator
-        # still spends its draws like the reference's.  Different sizes side by side = several handles (MixedFurnitureEnv).
-        self.resize_factor = None
-        if self.cfg.furn_size_rand != 0:
-            r = float(self.cfg.furn_size_rand)
-            self.resize_factor = 1 + float(np.random.RandomState(int(self.cfg.seed)).uniform(-r, r, 1)[0])
-        if control_type in NEW_CONTROLLERS:
-            if agent != "Sawyer":
-                raise NotImplementedError("the torque controllers are built for the Sawyer env")
-            agent = "SawyerTorque"  # robots/sawyer/robot_torque.xml (furniture.py:1893-1899)
-        self.model = mjcf.load_scene(agent, furniture_name, resize_factor=self.resize_factor)
-        self.dense_cfg = dense_config(**dense) if dense is not None else None
-        self.control_type = control_type
-        self.ik_cfg = None
-        if control_type in ("ik", "ik_quaternion"):
-            if agent not in ("Sawyer", "Baxter"):
-                raise NotImplementedError("control_type='%s' is built for the Sawyer and Baxter envs" % control_type)
-            from .ik import ik_config
-
-            self.ik_cfg = ik_config(self.model, **dict(ik or {}, quaternion_mode=int(control_type == "ik_quaternion")))
-        self.ctl_cfg = None
-        if control_type in NEW_CONTROLLERS:
-            from .controllers import ctl_config
-
-            self.ctl_cfg = ctl_config(control_type, model=self.model, move_speed=(ik or {}).get("move_speed", 0.1))
-        elif control_type not in ("impedance", "ik", "ik_quaternion"):
-            raise NotImplementedError("control_type %r is not built" % control_type)
-        self.obs_flags = dict(robot_ob=bool(robot_ob), object_ob=bool(object_ob), object_ob_all=bool(object_ob_all), subtask_ob=bool(subtask_ob))
-        self.engine = Engine(self.model, num_envs, device=device, config=self.cfg, dense=self.dense_cfg, ik=self.ik_cfg, controller=self.ctl_cfg,
-                             obs_layout=self.obs_flags, fix_init=fix_init, fix_init_parts=fix_init_parts, reset_robot_after_attach=reset_robot_after_attach)
-        self.num_envs = num_envs
-        self.obs_dim, self.act_dim = self.engine.obs_dim, self.engine.act_dim
-        self.n_objects = self.engine.scene.npart
-        # control_type="ik": robot_ob is gripper_qpos, eef_pos, eef_quat, eef_velp, eef_velr only -- no joint positions / velocities
-        # (furniture_sawyer.py:110-125); the device row always holds all of it, the 15 numbers are its tail (of each arm's block for two arms,
-        # furniture_baxter.py:137-160)
-        self._robot_skip = 0 if control_type == "impedance" else 14
-        self._narms = max(1, int(self.engine.scene.narms))
-        self._cols = obs_columns(self.engine.scene, self._robot_skip, **self.obs_flags)
-        width = lambda k: (len(range(self.obs_dim)[self._cols[k]]) if isinstance(self._cols[k], slice) else len(self._cols[k])) if k in self._cols else 0
-        self.object_ob_dim, self.subtask_ob_dim, self.robot_ob_dim, self.phase_ob_dim = (width(k) for k in ("object_ob", "subtask_ob", "robot_ob", "phase_ob"))
-        self._cols = OrderedDict((k, c if isinstance(c, slice) else torch.tensor(c, dtype=torch.long, device=self.device)) for k, c in self._cols.items())
-        self.dof = self.act_dim
+        self.engine = e = build_engine(agent, furniture_name, num_envs, device=device, **options)
+        self.model, self.cfg, self.dense_cfg, self.ik_cfg, self.ctl_cfg = e.model, e.cfg, e.dense, e.ik, e.controller
+        self.control_type, self.resize_factor, self.obs_flags = e.control_type, e.resize_factor, e.obs_flags
+        self.num_envs, self.obs_dim, self.act_dim, self.dof, self.n_objects = num_envs, e.obs_dim, e.act_dim, e.act_dim, e.scene.npart
+        cols, widths = e.obs_columns()
+        self.object_ob_dim, self.subtask_ob_dim, self.robot_ob_dim, self.phase_ob_dim = (widths[k] for k in ("object_ob", "subtask_ob", "robot_ob", "phase_ob"))
+        self._cols = OrderedDict((k, c if isinstance(c, slice) else torch.tensor(c, dtype=torch.long, device=self.device)) for k, c in cols.items())
         self._obs = torch.empty((num_envs, self.obs_dim), dtype=torch.float32, device=self.device)
         self._rew = torch.empty(num_envs, dtype=torch.float32, device=self.device)
         self._done = torch.empty(num_envs, dtype=torch.uint8, device=self.device)
         self._info = torch.empty((num_envs, INFO_DIM), dtype=torch.int32, device=self.device)
         self._act = torch.empty((num_envs, self.act_dim), dtype=torch.float32, device=self.device)
-        if prefix_length(preassembled) or num_connects is not None:
-            self.set_subtask(prefix_length(preassembled), num_connects)
-        apply_init_config(self, load_init_states, load_demo)
 
     def set_init_qpos(self, states):
         """FurnitureEnv.set_init_qpos (furniture.py:315-316), per env: one get_env_state dict or None for all envs, or a list of num_envs of
@@ -319,17 +334,11 @@ class BatchedFurnitureEnv:
 def make_vec_env(env_id="IKEASawyer-v0", num_env=1, config=None, device=0):
     """make_vec_env(env_id, num_env, config) of furniture/env/base.py:55-80: `config` may be the reference's argparse
     Namespace (config/furniture.py) or a dict; options outside the accelerated path are ignored (listed in `.ignored_config`)."""
-    agent = ENV_IDS.get(env_id)
-    if agent is None:
+    if env_id not in ENV_IDS:
         raise ValueError("unknown env id %s (this build accelerates %s)" % (env_id, sorted(ENV_IDS)))
-    ctl = control_options(config)
-    if env_id in DENSE_IDS:
-        furniture, over, dense, ignored = split_dense_config(config)
-        env = BatchedFurnitureEnv(agent, furniture, num_env, device=device, dense=dense, **ctl, **over)
-    else:
-        furniture, over, ignored = split_config(config)
-        env = BatchedFurnitureEnv(agent, furniture, num_env, device=device, **ctl, **over)
-    ignored = [k for k in ignored if k not in ("move_speed", "rotate_speed")] if "ik" in ctl else ignored
+    agent, dense_reward = ENV_IDS[env_id]
+    furniture, options, ignored = env_options(config, dense_reward)
+    env = BatchedFurnitureEnv(agent, furniture, num_env, device=device, **options)
     env.ignored_config = ignored
     return env
 

@@ -20,11 +20,6 @@ from collections import OrderedDict
 
 import numpy as np
 
-from . import mjcf
-from .engine import OBS_DEFAULTS, Engine, default_config, obs_columns
-
-AGENTS = {"FurnitureSawyerDenseRewardEnv": "Sawyer", "IKEASawyerDense-v0": "Sawyer", "furniture-sawyer-densereward-v0": "Sawyer", "FurnitureSawyerEnv": "Sawyer", "IKEASawyer-v0": "Sawyer", "Sawyer": "Sawyer", "FurnitureBaxterEnv": "Baxter", "IKEABaxter-v0": "Baxter", "Baxter": "Baxter"}
-
 
 class FurnitureGymB200:
     metadata = {"render.modes": []}
@@ -32,59 +27,25 @@ class FurnitureGymB200:
     def __init__(self, name="FurnitureSawyerEnv", furniture_name=None, device=0, lib_path=None, id=None, **config):
         """`id`, `name` and the remaining keywords are what gym passes from the registration (env/__init__.py:19-114: id, name,
         furniture_name / furniture_id, background, port ...); options of the renderer are ignored, see env.split_config"""
-        from .dense import dense_config
-        from .env import DENSE_IDS, NEW_CONTROLLERS, RESET_DEFAULTS, apply_init_config, control_options, prefix_length, split_config, split_dense_config
+        from .env import ENV_IDS, build_engine, env_options
 
-        if name not in AGENTS:
-            raise ValueError("unknown env %s (this build accelerates %s)" % (name, sorted(AGENTS)))
+        ids = dict(ENV_IDS, Sawyer=ENV_IDS["FurnitureSawyerEnv"], Baxter=ENV_IDS["FurnitureBaxterEnv"])  # and the bare agent names
+        if name not in ids:
+            raise ValueError("unknown env %s (this build accelerates %s)" % (name, sorted(ids)))
         if furniture_name is not None:
             config["furniture_name"] = furniture_name
-        self.dense_cfg = None
-        if name in DENSE_IDS:  # FurnitureSawyerDenseRewardEnv: the phase-based reward, computed inside the step kernel
-            furniture_name, over, dense, self.ignored_config = split_dense_config(config)
-            self.dense_cfg = dense_config(**dense)
-        else:
-            furniture_name, over, self.ignored_config = split_config(config)
-        preassembled, num_connects = prefix_length(over.pop("preassembled", None)), over.pop("num_connects", None)
-        load_init_states, load_demo = over.pop("load_init_states", None), over.pop("load_demo", None)
-        self.obs_flags = dict(OBS_DEFAULTS, **{k: over.pop(k) for k in OBS_DEFAULTS if k in over})  # robot_ob ... subtask_ob (furniture.py:103-107)
-        reset_options = {k: over.pop(k) for k in RESET_DEFAULTS if k in over}  # fix_init, fix_init_parts, reset_robot_after_attach
-        ctl = control_options(config)
-        self.control_type, self.ik_cfg, self.ctl_cfg = ctl["control_type"], None, None
-        agent = AGENTS[name]
-        if self.control_type in NEW_CONTROLLERS:  # the torque controllers run on the torque-actuated robot (furniture.py:1893-1899)
-            if agent != "Sawyer":
-                raise NotImplementedError("the torque controllers are built for the Sawyer env")
-            agent = "SawyerTorque"
-        self.model = mjcf.load_scene(agent, furniture_name)
-        self.cfg = default_config(**over)
-        if self.control_type in NEW_CONTROLLERS:
-            from .controllers import ctl_config
-
-            self.ctl_cfg = ctl_config(self.control_type, model=self.model, move_speed=ctl.get("ik", {}).get("move_speed", 0.1))
-        if self.control_type in ("ik", "ik_quaternion"):  # "ik" is the reference's default control type (config/furniture.py:57)
-            if AGENTS[name] not in ("Sawyer", "Baxter"):
-                raise NotImplementedError("control_type='%s' is built for the Sawyer and Baxter envs" % self.control_type)
-            from .ik import ik_config
-
-            self.ik_cfg = ik_config(self.model, **dict(ctl["ik"], quaternion_mode=int(self.control_type == "ik_quaternion")))
-        self.engine = Engine(self.model, 1, device=device, config=self.cfg, lib_path=lib_path, dense=self.dense_cfg, ik=self.ik_cfg, controller=self.ctl_cfg,
-                             obs_layout=self.obs_flags, **reset_options)
-        self.n_objects = self.engine.scene.npart
-        self._robot_skip = 0 if self.control_type == "impedance" else 14  # ik: robot_ob has no joint positions / velocities (furniture_sawyer.py:110-125)
-        self._narms = max(1, int(self.engine.scene.narms))
-        cols = obs_columns(self.engine.scene, self._robot_skip, **self.obs_flags)
-        self._cols = OrderedDict((k, np.arange(self.engine.obs_dim)[c]) for k, c in cols.items())  # the row's columns of each obs entry
-        width = lambda k: len(self._cols[k]) if k in self._cols else 0
-        self.object_ob_dim, self.subtask_ob_dim, self.robot_ob_dim, self.phase_ob_dim = (width(k) for k in ("object_ob", "subtask_ob", "robot_ob", "phase_ob"))
-        self.dof = self.engine.act_dim
+        agent, dense_reward = ids[name]
+        furniture_name, options, self.ignored_config = env_options(config, dense_reward)
+        self.engine = e = build_engine(agent, furniture_name, 1, device=device, lib_path=lib_path, **options)
+        self.model, self.cfg, self.dense_cfg, self.ik_cfg, self.ctl_cfg = e.model, e.cfg, e.dense, e.ik, e.controller
+        self.control_type, self.obs_flags, self.n_objects, self.dof = e.control_type, e.obs_flags, e.scene.npart, e.act_dim
+        cols, widths = e.obs_columns()
+        self._cols = OrderedDict((k, np.arange(e.obs_dim)[c]) for k, c in cols.items())  # the row's columns of each obs entry
+        self.object_ob_dim, self.subtask_ob_dim, self.robot_ob_dim, self.phase_ob_dim = (widths[k] for k in ("object_ob", "subtask_ob", "robot_ob", "phase_ob"))
         self._max_episode_steps = self.cfg.max_episode_steps
         self._pending_ob = None  # observation of an episode the device has already started
         self._episode_reward = 0.0
         self._episode_time = time.time()
-        if preassembled or num_connects is not None:
-            self.set_subtask(preassembled, num_connects)
-        apply_init_config(self, load_init_states, load_demo)
 
     # ---- spaces (furniture.py:215-252, :293-310): plain shape / bound records, gym.spaces objects when gym is installed
     @property
