@@ -241,8 +241,11 @@ FE_FN void fe_env_ctl_step_one(FeEnv* e, FeCtlArgs ctl, const float* action, flo
       fe_env_clear_flags(e);
     }
   LANES_END
+  fe_env_agent_masks(e);
   fe_forward(w); // sim.forward() ahead of the loop (:3080): the first _pre_action reads fresh kinematics
-  for (int i = 0; i < e->cfg->nsub; ++i) {
+  const int n = e->es.substeps[e->env];
+  for (int i = 0; fe_block_any(i < n); ++i) {
+    if (i >= n) { fe_substep_idle(); continue; }
     LANES_BEGIN
       if (lane == 0) {
         double arm[7] = {0, 0, 0, 0, 0, 0, 0}, tau[7];

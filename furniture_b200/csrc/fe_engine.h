@@ -2232,8 +2232,9 @@ FE_FN void fe_substep(FeWarp* w) {
   fe_integrate(w);
 }
 // same step with block barriers between the phases: the warps (= envs) of a block then fetch the same instructions at the
-// same time, which is what keeps the instruction cache effective for this large, mostly straight-line code.  Only legal
-// where every live warp of the block executes the same number of steps (the nsub loop of an env step).
+// same time, which is what keeps the instruction cache effective for this large, mostly straight-line code.  Every live warp
+// of the block must reach the same sequence of barriers: the step loops of the env steps, whose length is the env's own
+// substep count, keep it with fe_block_any and fe_substep_idle (below); fe_run_env runs one count for the whole launch.
 FE_FN void fe_substep_lockstep(FeWarp* w) {
   FE_TICK_START
   FE_BLOCK_SYNC; FE_TICK(w->u() + FE_U_STAT, FE_STAT_WAIT, FE_STAT_WAIT_KIN) fe_kin_smooth(w); FE_TICK(w->u() + FE_U_STAT, FE_STAT_KIN)
@@ -2246,3 +2247,18 @@ FE_FN void fe_substep_lockstep(FeWarp* w) {
   FE_TICK(w->u() + FE_U_STAT, FE_STAT_SOLVE)
   FE_BLOCK_SYNC; FE_TICK(w->u() + FE_U_STAT, FE_STAT_WAIT, FE_STAT_WAIT_INTEGRATE) fe_integrate(w); FE_TICK(w->u() + FE_U_STAT, FE_STAT_INTEGRATE)
 }
+// A step loop whose trip count differs between the warps of a block (each env's substeps) runs as
+//   for (int i = 0; fe_block_any(i < n); ++i) { if (i < n) fe_substep_lockstep(w); else fe_substep_idle(); }
+// Every live warp runs the block's largest count of iterations: one whose own steps are done passes the five barriers of a step
+// without the step.  The loop test is a barrier itself (bar.red.or on sm_90a), reached by every live thread once per iteration, and
+// its result is the same on every thread, so the block's threads all leave the loop after the same iteration and every barrier
+// phase sees all of them, each phase with one kind of barrier instruction.  Warps of empty slots exit before the first barrier,
+// as with a uniform count: an exited warp is no longer waited for.  `n` is equal on the lanes of a warp (one env per warp).
+FE_HD bool fe_block_any(bool p) {
+#if FE_DEVICE_BUILD
+  return __syncthreads_or(p ? 1 : 0) != 0;
+#else
+  return p; // the emulation runs one warp at a time
+#endif
+}
+FE_HD void fe_substep_idle() { FE_BLOCK_SYNC; FE_BLOCK_SYNC; FE_BLOCK_SYNC; FE_BLOCK_SYNC; FE_BLOCK_SYNC; }

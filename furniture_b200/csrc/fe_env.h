@@ -70,6 +70,8 @@ struct FeEnvState {
   double* fix_pose;                            // [N][npart][7] position, quaternion (w, x, y, z)
   int* reset_arm;                              // [N] reset_robot_after_attach (config/furniture.py:169-174)
   int* arm_resync;                             // [N] a connection sent the arm home: the next IK command re-seeds its position target
+  int* substeps;                               // [N] mj_steps of the env's step: int(control_timestep / model_timestep) (furniture.py:2878)
+  int* no_collision;                           // [N] 0 / 1: the agent's masks stay 0 (config/furniture.py no_collision, furniture.py:1962-1965)
   int *robot_contype, *robot_conaff;           // [N][ngeom] saved robot masks during reset
   float* episode_reward;
   // dense (phase-based) reward, fe_dense.h: NULL = the sparse reward of FurnitureEnv._compute_reward
@@ -77,6 +79,12 @@ struct FeEnvState {
   FeDenseState* dstate;                        // [N]
   float* dinfo;                                // [N][FE_DENSE_INFO]
 };
+
+// the geoms no_collision switches off.  The reference zeroes the masks of every geom under the robot's worldbody, grippers included
+// (furniture.py:1962-1965); among the geoms the engine keeps (those that can collide) that is every one that belongs to neither a furniture
+// part nor the floor: FE_TAG_ROBOT (the robot's contact geoms, which the reset switches off) and the agent's other colliding geoms
+// (the torque Sawyer's controller box and pedestal feet, Baxter's head, pedestal and left wrist)
+FE_BOTH bool fe_geom_is_agent(int tag) { return !(tag & FE_TAG_FLOOR) && ((tag >> FE_TAG_PART_SHIFT) & 0x3FFFFF) == 0; }
 
 // ---------------------------------------------------------------- float64 helpers with numpy's arithmetic
 #if FE_DEVICE_BUILD
@@ -668,6 +676,7 @@ FE_FN void fe_env_reset_clear(FeEnv* e, int pre) {
   const int nr = m->nr, np = m->npart, ng = m->ngeom;
   int* rct = e->es.robot_contype + (size_t)e->env * ng;
   int* rca = e->es.robot_conaff + (size_t)e->env * ng;
+  const bool off = e->es.no_collision[e->env] != 0;
   LANES_BEGIN
     // sim.reset(): data only (model arrays such as masks / eq_data persist)
     for (int i = lane; i < m->nq; i += 32) w->qpos()[i] = 0.f;
@@ -679,6 +688,7 @@ FE_FN void fe_env_reset_clear(FeEnv* e, int pre) {
       const int tag = m->geom_tag[g];
       if (tag & FE_TAG_ROBOT) { rct[g] = w->contype()[g]; rca[g] = w->conaff()[g]; w->contype()[g] = 0; w->conaff()[g] = 0; } // furniture.py:1441-1453
       if (tag & (1 << 30)) { w->contype()[g] = 1; w->conaff()[g] = 1; }                                                    // :1456-1461
+      if (off && fe_geom_is_agent(tag)) { w->contype()[g] = 0; w->conaff()[g] = 0; }                                     // no_collision (:1962-1965)
     }
     for (int q = lane; q < m->neq; q += 32) w->eq_active()[q] = 0; // :1501-1503
     for (int s = lane; s < m->nsite; s += 32) e->es.site_connected[(size_t)e->env * m->nsite + s] = 0;
@@ -763,6 +773,7 @@ FE_FN void fe_env_reset_robot(FeEnv* e) {
   const int ng = m->ngeom;
   const int* rct = e->es.robot_contype + (size_t)e->env * ng;
   const int* rca = e->es.robot_conaff + (size_t)e->env * ng;
+  const bool off = e->es.no_collision[e->env] != 0; // the masks the reset saved are the agent's zeros (furniture.py:1962-1965)
   // gravity compensation, robot pose, one step with robot collisions still off (furniture.py:1569-1584)
   for (int phase = 0; phase < 101; ++phase) {
     LANES_BEGIN
@@ -770,7 +781,7 @@ FE_FN void fe_env_reset_robot(FeEnv* e) {
         for (int i = lane; i < sc->narm; i += 32) w->qfrc_applied()[sc->arm_dof[i]] = w->bias()[sc->arm_dof[i]];
         for (int i = lane; i < sc->ngrip; i += 32) w->qfrc_applied()[sc->grip_dof[i]] = w->bias()[sc->grip_dof[i]];
       }
-      if (phase == 1) for (int g = lane; g < ng; g += 32) if (m->geom_tag[g] & FE_TAG_ROBOT) { w->contype()[g] = rct[g]; w->conaff()[g] = rca[g]; } // :1586-1595
+      if (phase == 1) for (int g = lane; g < ng; g += 32) if (m->geom_tag[g] & FE_TAG_ROBOT) { w->contype()[g] = off ? 0 : rct[g]; w->conaff()[g] = off ? 0 : rca[g]; } // :1586-1595
       if (lane == 0) fe_init_robot_pos(e);
     LANES_END
     fe_fwd_step(e);
@@ -817,6 +828,7 @@ FE_FN void fe_env_set_init_state(FeEnv* e, int s, bool robot) {
   const int ng = m->ngeom;
   const int* rct = e->es.robot_contype + (size_t)e->env * ng;
   const int* rca = e->es.robot_conaff + (size_t)e->env * ng;
+  const bool off = e->es.no_collision[e->env] != 0;
   const float* q = e->es.init_qpos + (size_t)s * m->nq;
   const float* v = e->es.init_qvel + (size_t)s * m->nv;
   LANES_BEGIN
@@ -824,7 +836,7 @@ FE_FN void fe_env_set_init_state(FeEnv* e, int s, bool robot) {
     for (int i = lane; i < m->nq; i += 32) w->qpos()[i] = q[i];
     for (int i = lane; i < m->nv; i += 32) w->qvel()[i] = v[i];
     for (int i = lane; i < m->nu; i += 32) w->ctrl()[i] = 0.f;
-    if (robot) for (int g = lane; g < ng; g += 32) if (m->geom_tag[g] & FE_TAG_ROBOT) { w->contype()[g] = rct[g]; w->conaff()[g] = rca[g]; }
+    if (robot) for (int g = lane; g < ng; g += 32) if (m->geom_tag[g] & FE_TAG_ROBOT) { w->contype()[g] = off ? 0 : rct[g]; w->conaff()[g] = off ? 0 : rca[g]; }
   LANES_END
 }
 // the pick before every reset (furniture.py:1433-1434): `if np.random.rand() > 0.2: set_init_qpos(np.random.choice(states))` over the first
@@ -874,6 +886,15 @@ FE_HD void fe_env_reset_unstable(FeEnv* e) {
   fe_env_reset_one(e);
 }
 
+// no_collision: the agent's masks stay 0 through the env's steps, whatever wrote them since (furniture.py:1962-1965)
+FE_HD void fe_env_agent_masks(FeEnv* e) {
+  if (!e->es.no_collision[e->env]) return;
+  FeWarp* w = e->w;
+  const fe_model* m = w->m;
+  LANES_BEGIN
+    for (int g = lane; g < m->ngeom; g += 32) if (fe_geom_is_agent(m->geom_tag[g])) { w->contype()[g] = 0; w->conaff()[g] = 0; }
+  LANES_END
+}
 // the per-step flags: no connection found, no re-pin pending, no auto-reset due, no simulation failure yet (lane 0)
 FE_HD void fe_env_clear_flags(FeEnv* e) { e->si->aligned = 0; e->si->repin = -1; e->si->done = 0; e->w->u()[FE_U_FLAGS] = 0; }
 
@@ -1020,7 +1041,11 @@ FE_FN void fe_env_step_one(FeEnv* e, const float* action, float* reward_out, uin
   if (cfg->discrete_grip) grip = grip < 0.f ? -1.f : 1.f; // FurnitureSawyerEnv._step only (furniture_sawyer.py:73-74); Baxter: index -1
   const float connect = a[sc->connect_action_index];
   fe_env_controls(e, a, grip);
-  for (int i = 0; i < cfg->nsub; ++i) fe_substep_lockstep(w); // _do_simulation, furniture.py:2877-2879
+  fe_env_agent_masks(e);
+  const int n = e->es.substeps[e->env];
+  for (int i = 0; fe_block_any(i < n); ++i) { // _do_simulation, furniture.py:2877-2879
+    if (i < n) fe_substep_lockstep(w); else fe_substep_idle();
+  }
   const int fail = (w->u()[FE_U_FLAGS] & FE_FLAG_DIVERGED) ? 1 : 0; // MujocoException path, :2889-2897
   fe_env_finish(e, a, sc->act_dim, connect, fail, fail, reward_out, done_out, info_out);
 }

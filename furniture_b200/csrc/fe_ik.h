@@ -221,6 +221,8 @@ FE_FN void fe_env_ik_step_one(FeEnv* e, FeIkArgs ik, const float* action, float*
     }
   LANES_END
   int fail = 0, reset_now = 0;
+  const int n = e->es.substeps[e->env];
+  fe_env_agent_masks(e);
   for (int r = 0; r < c->action_repeat; ++r) {
     if (r > 0) { // closed loop: get_control() without arguments, furniture.py:2988-2995
       LANES_BEGIN
@@ -228,7 +230,9 @@ FE_FN void fe_env_ik_step_one(FeEnv* e, FeIkArgs ik, const float* action, float*
       LANES_END
     }
     fe_env_controls(e, st->low, grip);
-    for (int i = 0; i < e->cfg->nsub; ++i) fe_substep_lockstep(w);
+    for (int i = 0; fe_block_any(i < n); ++i) {
+      if (i < n) fe_substep_lockstep(w); else fe_substep_idle();
+    }
     if (w->u()[FE_U_FLAGS] & FE_FLAG_DIVERGED) { // _do_simulation's except branch: reset, then the remaining repeats run on the new episode (furniture.py:2889-2897)
       fail = 1;
       FE_SYNC;

@@ -79,6 +79,20 @@ def default_config(**kw):
     return c
 
 
+def substep_count(control_freq, timestep):
+    """mj_steps of one env step at `control_freq` (a positive number, or an array of them): the bound of _do_simulation's loop,
+    int((1.0 / control_freq) / model.opt.timestep) (furniture.py:2855, :2878), in float64 with the model's float64 timestep as MuJoCo
+    holds it (a float32 timestep would give 49 at 10 Hz).  A frequency whose count is 0 (above 1 / timestep) is a ValueError."""
+    cf = np.asarray(control_freq, dtype=np.float64)
+    if not np.all(np.isfinite(cf)) or np.any(cf <= 0):
+        raise ValueError("control_freq must be a positive number, got %r" % (control_freq,))
+    dt = float(timestep)
+    n = np.array([int((1.0 / float(f)) / dt) for f in cf.ravel()], dtype=np.int64).reshape(cf.shape)
+    if np.any(n < 1):
+        raise ValueError("control_freq %r runs no mj_step per env step (timestep %g s: at most %g Hz)" % (control_freq, dt, 1.0 / dt))
+    return n
+
+
 def auto_maxcon(em: EngineModel) -> int:
     """Contact capacity per env when the config leaves it open.  The reference runs with nconmax=5000 (base.xml:5), i.e.
     never full; the engine keeps contacts in the env's shared-memory slice, so capacity is sized from the scene: four
@@ -320,6 +334,27 @@ class Engine:
             cur[idx, 0] = int(v)
             self.set(name, cur)
 
+    def substeps(self, control_freq):
+        """substep_count at this model's timestep"""
+        return substep_count(control_freq, self.model.opt_timestep)
+
+    def set_sim_options(self, control_freq=None, no_collision=None, envs=None):
+        """control_freq (config/furniture.py: mj_steps per env step, see substeps) and no_collision (the agent's contype = conaffinity = 0,
+        furniture.py:1962-1965) for the envs in `envs` (default: all), each a scalar or one value per env of `envs`; None leaves an option as
+        it is.  A new control_freq takes effect from the env's next step; no_collision changes the env's masks at once (back to the
+        model's compiled masks when it turns off)."""
+        if self.model.meta.get("agent") == "Cursor":
+            raise ValueError("the Cursor env takes its own control_freq (cursor_env.FurnitureCursorEnvB200); control_freq and no_collision "
+                             "are options of the robot envs")
+        idx = np.arange(self.N) if envs is None else np.asarray(envs, dtype=np.int64).ravel()
+        for name, v in (("substeps", None if control_freq is None else self.substeps(control_freq)),
+                        ("no_collision", None if no_collision is None else np.asarray(no_collision, dtype=bool).astype(np.int32))):
+            if v is None:
+                continue
+            cur = self.get(name)
+            cur[idx, 0] = v
+            self.set(name, cur)
+
     def close(self):
         if getattr(self, "h", None) and self.h.value:
             self.L.fe_destroy(self.h)
@@ -343,7 +378,8 @@ class Engine:
 
     _INT = {"order", "geom_contype", "geom_conaffinity", "eq_active", "touch", "flags", "ncon", "niter", "stats", "con_geom", "con_state", "group", "site_connected",
             "num_connected", "prev_num_connected", "touched", "picked", "episode_length", "done", "mt_pos", "preassembled", "num_connects",
-            "init_state", "init_pick", "init_mt_pos", "subtask_part", "fix_init", "fix_init_parts", "fix_have", "reset_robot_after_attach"}
+            "init_state", "init_pick", "init_mt_pos", "subtask_part", "fix_init", "fix_init_parts", "fix_have", "reset_robot_after_attach",
+            "substeps", "no_collision"}
     _U32 = {"mt_state", "init_mt_state"}
     _F64 = {"fix_pose"}
 

@@ -21,6 +21,7 @@ from .dense import DENSE_DEFAULTS, DENSE_ENV_DEFAULTS, INFO_KEYS as DENSE_INFO_K
 from .engine import INFO_DIM, OBS_DEFAULTS, Engine, default_config
 
 RESET_DEFAULTS = dict(fix_init=False, fix_init_parts=None, reset_robot_after_attach=False)  # config/furniture.py:116-127, :169-174
+SIM_DEFAULTS = dict(control_freq=10, no_collision=False)  # config/furniture.py:71-73, :304-306
 INFO_KEYS = ("num_connected", "episode_success", "episode_unstable", "episode_length", "ncon", "solver_iters")
 # env id or class name (env/__init__.py:19-114) -> (agent, whether it is FurnitureSawyerDenseRewardEnv, env/__init__.py:103-114)
 ENV_IDS = {"IKEASawyer-v0": ("Sawyer", False), "FurnitureSawyerEnv": ("Sawyer", False), "IKEABaxter-v0": ("Baxter", False),
@@ -54,8 +55,9 @@ def split_config(config):
     `furniture_name` wins over `furniture_id` as in furniture.py:157-161; keys the accelerated path has no use for (port, background,
     camera and rendering options, the speeds where no control type reads them ...) are returned so that callers can report them instead of
     failing on them.  `preassembled` (checked to be a recipe prefix), `num_connects`, `load_init_states`, `load_demo` and the observation flags
-    `robot_ob`, `object_ob`, `object_ob_all`, `subtask_ob` and the reset options `fix_init`, `fix_init_parts`, `reset_robot_after_attach` travel
-    with the overrides when they are set (the flags when they differ from their defaults): they are keywords of build_engine."""
+    `robot_ob`, `object_ob`, `object_ob_all`, `subtask_ob`, the reset options `fix_init`, `fix_init_parts`, `reset_robot_after_attach` and
+    `control_freq`, `no_collision` travel with the overrides when they are set (the flags when they differ from their defaults): they are
+    keywords of build_engine."""
     from .engine import FeConfig
 
     cfg = dict(vars(config)) if hasattr(config, "__dict__") and not isinstance(config, dict) else dict(config or {})
@@ -71,7 +73,8 @@ def split_config(config):
     renamed = {"furn_xyz_rand": "furn_xyz_rand", "furn_rot_rand": "furn_rot_rand", "agent_xyz_rand": "agent_xyz_rand", "alignment_pos_dist": "alignment_pos_dist"}
     over = {renamed.get(k, k): v for k, v in cfg.items() if renamed.get(k, k) in fields and v is not None}
     ignored = sorted(k for k in cfg if k not in over and k not in ("furniture_name", "furniture_id", "control_type", "preassembled", "num_connects",
-                                                                   "load_init_states", "load_demo") + tuple(OBS_DEFAULTS) + tuple(RESET_DEFAULTS))
+                                                                   "load_init_states", "load_demo") + tuple(OBS_DEFAULTS) + tuple(RESET_DEFAULTS)
+                     + tuple(SIM_DEFAULTS))
     if "ik" in control_options(cfg):  # the speeds reach the IK or the controller
         ignored = [k for k in ignored if k not in ("move_speed", "rotate_speed")]
     if prefix_length(cfg.get("preassembled")):
@@ -87,6 +90,10 @@ def split_config(config):
     for k in RESET_DEFAULTS:  # config/furniture.py:116-127, :169-174; False, None and the empty set are the defaults
         if cfg.get(k):
             over[k] = cfg[k] if k == "fix_init_parts" else bool(cfg[k])
+    if cfg.get("control_freq") is not None and cfg["control_freq"] != SIM_DEFAULTS["control_freq"]:  # furniture.py:84, :2855, :2878
+        over["control_freq"] = cfg["control_freq"]
+    if cfg.get("no_collision"):  # furniture.py:1962-1965
+        over["no_collision"] = bool(cfg["no_collision"])
     return name or "table_lack_0825", over, ignored
 
 
@@ -142,7 +149,7 @@ def env_options(config, dense_reward=False):
 
 def build_engine(agent, furniture_name, num_envs, device=0, lib_path=None, dense=None, control_type="impedance", ik=None, preassembled=None,
                  num_connects=None, load_init_states=None, load_demo=None, robot_ob=True, object_ob=True, object_ob_all=True, subtask_ob=False,
-                 fix_init=False, fix_init_parts=None, reset_robot_after_attach=None, **cfg_overrides):
+                 fix_init=False, fix_init_parts=None, reset_robot_after_attach=None, control_freq=None, no_collision=False, **cfg_overrides):
     """The Engine of `num_envs` envs of `agent` + `furniture_name` that both env surfaces run; `lib_path` as for Engine.  The keywords:
         `dense`: None for the sparse reward of FurnitureEnv; a dict of coefficient overrides (possibly empty) for the phase-based
         reward of FurnitureSawyerDenseRewardEnv, computed inside the step kernel (furniture_b200/dense.py).
@@ -161,7 +168,14 @@ def build_engine(agent, furniture_name, num_envs, device=0, lib_path=None, dense
         left); subtask_ob=True adds their part ids + 1 (float32).  Each env's pair follows its connections and resets inside the kernels.
         `fix_init`, `fix_init_parts`, `reset_robot_after_attach`: config/furniture.py:116-127, :169-174 (see set_reset_options).  A dense env
         takes reset_robot_after_attach from `dense`, whose phase machine follows it (None: off, or the dense reward's).
+        `control_freq`, `no_collision`: config/furniture.py's (see set_sim_options), a value for every env or one per env.  control_freq sets
+        the mj_steps of an env step (None: FeConfig.nsub, 50 = 10 Hz); it cannot be given together with an `nsub` override.
     The other keywords override FeConfig fields (default_config).  The engine records `control_type` and `resize_factor`."""
+    if control_freq is not None and "nsub" in cfg_overrides:
+        raise ValueError("control_freq and nsub both set the mj_steps of an env step: give one of them")
+    if agent == "Cursor" and (control_freq is not None or np.any(no_collision)):
+        raise ValueError("the Cursor env takes its own control_freq (cursor_env.FurnitureCursorEnvB200); control_freq and no_collision "
+                         "are options of the robot envs")
     cfg = default_config(**cfg_overrides)
     # furn_size_rand (config/furniture.py:196-201): the reference draws one size factor per env process while loading the model.
     # A handle shares one model: the batch takes env 0's factor (the first draw of RandomState(seed)); every env's generator
@@ -194,6 +208,8 @@ def build_engine(agent, furniture_name, num_envs, device=0, lib_path=None, dense
                     ik=ik_cfg, controller=ctl_cfg, obs_layout=obs_flags, fix_init=fix_init, fix_init_parts=fix_init_parts,
                     reset_robot_after_attach=reset_robot_after_attach)
     engine.control_type, engine.resize_factor = control_type, resize_factor
+    if control_freq is not None or np.any(no_collision):
+        engine.set_sim_options(control_freq=control_freq, no_collision=no_collision if np.any(no_collision) else None)
     if prefix_length(preassembled) or num_connects is not None:
         engine.set_subtask(prefix_length(preassembled), num_connects)
     apply_init_config(engine, load_init_states, load_demo)
@@ -247,6 +263,13 @@ class BatchedFurnitureEnv:
         names, or a comma string) does so for those parts only and places the others around them, reset_robot_after_attach sends the arm back
         to its start pose, with fresh noise, after every connection (furniture.py:916-924, :1389-1404, :1519-1532)"""
         self.engine.set_reset_options(fix_init, fix_init_parts, reset_robot_after_attach, envs)
+
+    def set_sim_options(self, control_freq=None, no_collision=None, envs=None):
+        """per env (`envs`, default: all; a scalar or one value per env of `envs`; None leaves an option as it is): control_freq sets the
+        mj_steps of the env's next steps to int((1 / control_freq) / timestep) (furniture.py:2855, :2878), no_collision switches every
+        collision of the agent off at once (furniture.py:1962-1965), or back on with the model's masks.  Envs at different frequencies
+        step together in one launch."""
+        self.engine.set_sim_options(control_freq, no_collision, envs)
 
     def set_subtask(self, subtask, num_connects=None):
         """FurnitureEnv.set_subtask (furniture.py:204-207) with a scalar or an (N,) array each, so that the envs of one batch can train different
@@ -393,6 +416,17 @@ class MixedFurnitureEnv:
         self._info = torch.empty((off, INFO_DIM), dtype=torch.int32, device=self.device)
         self._act = torch.empty((off, self.act_dim), dtype=torch.float32, device=self.device)
         self._streams = [torch.cuda.Stream(device=self.device) for _ in self.buckets]
+
+    def set_sim_options(self, control_freq=None, no_collision=None, envs=None):
+        """BatchedFurnitureEnv.set_sim_options with `envs` as global indices of this batch (default: all); each value is a scalar or one
+        per env of `envs`"""
+        idx = np.arange(self.real_envs) if envs is None else np.asarray(envs, dtype=np.int64).ravel()
+        per = lambda v: None if v is None else np.broadcast_to(np.asarray(v), idx.shape)
+        cf, nc = per(control_freq), per(no_collision)
+        for b, off in zip(self.buckets, self.offsets):
+            sel = (idx >= off) & (idx < off + b.num_envs)
+            if sel.any():
+                b.set_sim_options(None if cf is None else cf[sel], None if nc is None else nc[sel], idx[sel] - off)
 
     def _obs_dict(self, obs):
         d, o = OrderedDict(), 0

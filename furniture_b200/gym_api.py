@@ -120,6 +120,11 @@ class FurnitureGymB200:
     def num_subtask(self):
         return int(self.engine.num_subtask()[0])
 
+    def set_sim_options(self, control_freq=None, no_collision=None):
+        """config/furniture.py's control_freq (mj_steps of the next steps, furniture.py:2855, :2878) and no_collision (the agent's collisions
+        off at once, furniture.py:1962-1965); None leaves an option as it is"""
+        self.engine.set_sim_options(control_freq, no_collision)
+
     def set_init_qpos(self, init_qpos):
         """furniture.py:315-316 (FurnitureGym, furniture_gym.py:43): from the next reset on, episodes start from this get_env_state dict, or
         from random placement for None"""

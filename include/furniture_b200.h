@@ -43,7 +43,7 @@ typedef struct fe_config {
   int32_t newton_iters;      /* max Newton iterations per mj_step (MuJoCo default 100) */
   int32_t ls_iters;          /* max line-search evaluations per Newton iteration */
   float tolerance;           /* solver tolerance on scaled improvement / gradient (MuJoCo: 1e-8 in double) */
-  int32_t nsub;              /* mj_steps per env step = int(control_timestep / model_timestep), furniture.py:2878 */
+  int32_t nsub;              /* mj_steps per env step = int(control_timestep / model_timestep), furniture.py:2878: every env's substeps at fe_create */
   int32_t max_episode_steps; /* config/furniture.py:164 */
   int32_t discrete_grip, rescale_actions, auto_align; /* config/furniture.py:75, :90, :96 */
   double alignment_pos_dist, alignment_rot_dist_up, alignment_rot_dist_forward, alignment_project_dist; /* :203-226 */
@@ -110,7 +110,13 @@ int fe_sim_step(fe_handle* h, int nsub, void* stream);
    per part, XML order, read/write: position and quaternion w, x, y, z, the reference's init_pos / init_quat; fe_create leaves fix_have = 0,
    the XML poses are the caller's to seed); reset_robot_after_attach (int32, one per env, read/write: every connection, the reset's
    preassembly included, ends with _initialize_robot_pos, furniture.py:916-924, and the IK step re-seeds its position target; a dense handle
-   sets it from fe_dense_config.reset_robot_after_attach).  fe_set_field refuses flags outside {0, 1}, fix_init_parts bits at or beyond the
+   sets it from fe_dense_config.reset_robot_after_attach); substeps (int32, one per env, read/write: the env's mj_steps per env step,
+   int(control_timestep / model_timestep) of furniture.py:2878 for its control_freq; fe_create sets fe_config.nsub.  The stock step runs it,
+   the IK step runs it once per closed-loop repeat, the torque-controller step evaluates the controller before each of them; envs with
+   different counts share one launch); no_collision (int32, one per env, read/write: config/furniture.py's no_collision, furniture.py:1962-1965:
+   while 1, contype = conaffinity = 0 on every geom of the agent -- every colliding geom that is neither a furniture part's nor the floor --
+   through steps and resets.  Writing it changes the env's geom_contype / geom_conaffinity at once: 0 where it turns on, the model's compiled
+   masks where it turns off).  fe_set_field refuses flags outside {0, 1}, substeps below 1, fix_init_parts bits at or beyond the
    number of parts, non-finite fix_pose values or zero quaternions, fix_have = 1 for an env whose fix_pose was never written and, in a dense
    handle, a reset_robot_after_attach that differs from the dense reward's */
 int fe_get_field(fe_handle* h, const char* name, void* dst_host, size_t bytes);
