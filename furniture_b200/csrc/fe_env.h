@@ -72,6 +72,7 @@ struct FeEnvState {
   int* arm_resync;                             // [N] a connection sent the arm home: the next IK command re-seeds its position target
   int* substeps;                               // [N] mj_steps of the env's step: int(control_timestep / model_timestep) (furniture.py:2878)
   int* no_collision;                           // [N] 0 / 1: the agent's masks stay 0 (config/furniture.py no_collision, furniture.py:1962-1965)
+  int* assembled;                              // [N] 0 / 1: episodes start with every weld on, the parts at qpos0 (config/furniture.py:307-312)
   int *robot_contype, *robot_conaff;           // [N][ngeom] saved robot masks during reset
   float* episode_reward;
   // dense (phase-based) reward, fe_dense.h: NULL = the sparse reward of FurnitureEnv._compute_reward
@@ -690,7 +691,8 @@ FE_FN void fe_env_reset_clear(FeEnv* e, int pre) {
       if (tag & (1 << 30)) { w->contype()[g] = 1; w->conaff()[g] = 1; }                                                    // :1456-1461
       if (off && fe_geom_is_agent(tag)) { w->contype()[g] = 0; w->conaff()[g] = 0; }                                     // no_collision (:1962-1965)
     }
-    for (int q = lane; q < m->neq; q += 32) w->eq_active()[q] = 0; // :1501-1503
+    const int weld = e->es.assembled[e->env];
+    for (int q = lane; q < m->neq; q += 32) w->eq_active()[q] = weld; // :1501-1503: 1 if assembled else 0, eq_data kept as the model holds it
     for (int s = lane; s < m->nsite; s += 32) e->es.site_connected[(size_t)e->env * m->nsite + s] = 0;
     if (lane == 0) {
       e->es.num_connected[e->env] = 0; e->es.prev_num_connected[e->env] = 0; e->es.episode_len[e->env] = 0; e->es.episode_reward[e->env] = 0.f;
@@ -708,7 +710,8 @@ FE_FN void fe_env_reset_clear(FeEnv* e, int pre) {
 }
 // _place_objects and the first settle loop (:1519-1540).  The env's remembered placement fix_pose is the reference's init_pos / init_quat:
 // with fix_init and a placement held, the parts start there and nothing is drawn (:1522); otherwise the sampler runs and its placement is
-// remembered (:1520-1525), the parts of fix_init_parts planted at their remembered pose and placed first (:1397-1404) once there is one
+// remembered (:1520-1525), the parts of fix_init_parts planted at their remembered pose and placed first (:1397-1404) once there is one.
+// Under assembled the sampler still draws and init_pos is still updated, but no part is moved (:1526-1532): they stay at qpos0, in group 0
 FE_FN void fe_env_reset_place(FeEnv* e) {
   FeWarp* w = e->w;
   const fe_model* m = w->m;
@@ -761,6 +764,13 @@ FE_FN void fe_env_reset_place(FeEnv* e) {
       }
       e->es.fix_have[env] = 1;
       e->es.mt_pos[env] = pos;
+      if (e->es.assembled[env]) // `if self._config.assembled: self._object_group[i] = 0` instead of _set_qpos
+        for (int p = 0; p < np; ++p) { // qpos0 of a part's free joint is its link frame at qpos0, which the model holds (engine_model.py)
+          const int qa = m->link_qadr[nrl + p];
+          for (int k = 0; k < 3; ++k) w->qpos()[qa + k] = m->link_pos[nrl + p][k];
+          for (int k = 0; k < 4; ++k) w->qpos()[qa + 3 + k] = m->link_quat[nrl + p][k];
+          e->group[p] = 0;
+        }
     }
   LANES_END
   fe_env_stabilise(e);

@@ -196,6 +196,8 @@ class FurnitureCursorEnvB200:
             furniture_name = FURNITURE_NAMES[int(furniture_id)]
         if ignored.get("no_collision"):
             raise ValueError("no_collision is built for the robot envs, not the Cursor env")
+        if ignored.get("assembled"):
+            raise ValueError("assembled is built for the robot envs, not the Cursor env")
         self.ignored_config = sorted(ignored)
         self.model = m = backend.model if backend is not None else mjcf.load_scene("Cursor", furniture_name)
         self.sim = backend if backend is not None else EngineBackend(m, device=device, lib_path=lib_path)

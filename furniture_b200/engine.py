@@ -236,9 +236,9 @@ def obs_columns(scene, robot_skip=0, robot_ob=True, object_ob=True, object_ob_al
 class Engine:
     def __init__(self, model: mjcf.Model, n_envs: int, device: int = 0, config: FeConfig | None = None, lib_path: str | None = None,
                  dense: FeDenseConfig | None = None, ik=None, controller=None, obs_layout=None, fix_init=False, fix_init_parts=None,
-                 reset_robot_after_attach=None):
-        """`fix_init`, `fix_init_parts`, `reset_robot_after_attach`: the keys of config/furniture.py:116-127, :169-174 for every env of the
-        handle (set_reset_options changes them per env).  In a dense handle the dense reward's reset_robot_after_attach decides (None: follow it)."""
+                 reset_robot_after_attach=None, assembled=False):
+        """`fix_init`, `fix_init_parts`, `reset_robot_after_attach`, `assembled`: the keys of config/furniture.py:116-127, :169-174, :307-312
+        for every env of the handle (set_reset_options changes them per env).  In a dense handle the dense reward's reset_robot_after_attach decides (None: follow it)."""
         path = lib_path or DEFAULT_LIB
         if not os.path.exists(path):
             raise RuntimeError(
@@ -300,8 +300,8 @@ class Engine:
                 raise ValueError("reset_robot_after_attach=%r disagrees with the dense reward's %r, which drives the phase machine and the arm"
                                  % (rra, bool(dense.reset_robot_after_attach)))
             rra = None
-        if fix_init or fix_init_parts or rra:
-            self.set_reset_options(fix_init=fix_init, fix_init_parts=fix_init_parts, reset_robot_after_attach=rra)
+        if fix_init or fix_init_parts or rra or assembled:
+            self.set_reset_options(fix_init=fix_init, fix_init_parts=fix_init_parts, reset_robot_after_attach=rra, assembled=assembled or None)
 
     @staticmethod
     def _part_names(parts):
@@ -316,18 +316,21 @@ class Engine:
             raise ValueError("fix_init_parts names %s, which %s does not have (parts: %s)" % (unknown, self.model.meta.get("furniture"), list(self.em.part_names)))
         return sum(1 << self.em.part_names.index(n) for n in set(names))
 
-    def set_reset_options(self, fix_init=None, fix_init_parts=None, reset_robot_after_attach=None, envs=None):
+    def set_reset_options(self, fix_init=None, fix_init_parts=None, reset_robot_after_attach=None, envs=None, assembled=None):
         """fix_init (the furniture starts every episode where the env's first random placement, or the XML, put it: furniture.py:1519-1532),
-        fix_init_parts (only those parts do, the sampler places the others around them: :1389-1404) and reset_robot_after_attach (the arm goes
-        back to its start pose after every connection: :916-924), for the envs in `envs` (default: all); None leaves an option as it is.
+        fix_init_parts (only those parts do, the sampler places the others around them: :1389-1404), reset_robot_after_attach (the arm goes
+        back to its start pose after every connection: :916-924) and assembled (every weld on, the parts left at the model's qpos0 -- the
+        furniture as assembled -- in one group: :1501-1532), for the envs in `envs` (default: all); None leaves an option as it is.
         They act from the env's next reset or connection on, inside the kernels."""
+        if assembled is not None and self.model.meta.get("agent") == "Cursor":
+            raise ValueError("assembled is built for the robot envs; the Cursor env's reset is host logic (cursor_env.FurnitureCursorEnvB200)")
         partial = self._xml_listed and self._xml_listed != set(self.em.part_names)
         if partial and (fix_init or set(self._part_names(fix_init_parts)) - self._xml_listed):  # init_pos[body]: the reference's KeyError
             raise ValueError("the XML of %s lists init poses for some parts only: fix_init, and fix_init_parts beyond %s, are undefined there"
                              % (self.model.meta.get("furniture"), sorted(self._xml_listed)))
         idx = np.arange(self.N) if envs is None else np.asarray(envs, dtype=np.int64).ravel()
         for name, v in (("fix_init", fix_init), ("fix_init_parts", None if fix_init_parts is None else self.part_mask(fix_init_parts)),
-                        ("reset_robot_after_attach", reset_robot_after_attach)):
+                        ("reset_robot_after_attach", reset_robot_after_attach), ("assembled", assembled)):
             if v is None:
                 continue
             cur = self.get(name)
@@ -379,7 +382,7 @@ class Engine:
     _INT = {"order", "geom_contype", "geom_conaffinity", "eq_active", "touch", "flags", "ncon", "niter", "stats", "con_geom", "con_state", "group", "site_connected",
             "num_connected", "prev_num_connected", "touched", "picked", "episode_length", "done", "mt_pos", "preassembled", "num_connects",
             "init_state", "init_pick", "init_mt_pos", "subtask_part", "fix_init", "fix_init_parts", "fix_have", "reset_robot_after_attach",
-            "substeps", "no_collision"}
+            "substeps", "no_collision", "assembled"}
     _U32 = {"mt_state", "init_mt_state"}
     _F64 = {"fix_pose"}
 

@@ -20,7 +20,7 @@ from . import mjcf
 from .dense import DENSE_DEFAULTS, DENSE_ENV_DEFAULTS, INFO_KEYS as DENSE_INFO_KEYS, dense_config
 from .engine import INFO_DIM, OBS_DEFAULTS, Engine, default_config
 
-RESET_DEFAULTS = dict(fix_init=False, fix_init_parts=None, reset_robot_after_attach=False)  # config/furniture.py:116-127, :169-174
+RESET_DEFAULTS = dict(fix_init=False, fix_init_parts=None, reset_robot_after_attach=False, assembled=False)  # config/furniture.py:116-127, :169-174, :307-312
 SIM_DEFAULTS = dict(control_freq=10, no_collision=False)  # config/furniture.py:71-73, :304-306
 INFO_KEYS = ("num_connected", "episode_success", "episode_unstable", "episode_length", "ncon", "solver_iters")
 # env id or class name (env/__init__.py:19-114) -> (agent, whether it is FurnitureSawyerDenseRewardEnv, env/__init__.py:103-114)
@@ -55,7 +55,7 @@ def split_config(config):
     `furniture_name` wins over `furniture_id` as in furniture.py:157-161; keys the accelerated path has no use for (port, background,
     camera and rendering options, the speeds where no control type reads them ...) are returned so that callers can report them instead of
     failing on them.  `preassembled` (checked to be a recipe prefix), `num_connects`, `load_init_states`, `load_demo` and the observation flags
-    `robot_ob`, `object_ob`, `object_ob_all`, `subtask_ob`, the reset options `fix_init`, `fix_init_parts`, `reset_robot_after_attach` and
+    `robot_ob`, `object_ob`, `object_ob_all`, `subtask_ob`, the reset options `fix_init`, `fix_init_parts`, `reset_robot_after_attach`, `assembled` and
     `control_freq`, `no_collision` travel with the overrides when they are set (the flags when they differ from their defaults): they are
     keywords of build_engine."""
     from .engine import FeConfig
@@ -87,7 +87,7 @@ def split_config(config):
     for k, default in OBS_DEFAULTS.items():  # furniture.py:103-107; a flag at its default changes nothing and is not passed on
         if cfg.get(k) is not None and bool(cfg[k]) != default:
             over[k] = bool(cfg[k])
-    for k in RESET_DEFAULTS:  # config/furniture.py:116-127, :169-174; False, None and the empty set are the defaults
+    for k in RESET_DEFAULTS:  # config/furniture.py:116-127, :169-174, :307-312; False, None and the empty set are the defaults
         if cfg.get(k):
             over[k] = cfg[k] if k == "fix_init_parts" else bool(cfg[k])
     if cfg.get("control_freq") is not None and cfg["control_freq"] != SIM_DEFAULTS["control_freq"]:  # furniture.py:84, :2855, :2878
@@ -149,7 +149,8 @@ def env_options(config, dense_reward=False):
 
 def build_engine(agent, furniture_name, num_envs, device=0, lib_path=None, dense=None, control_type="impedance", ik=None, preassembled=None,
                  num_connects=None, load_init_states=None, load_demo=None, robot_ob=True, object_ob=True, object_ob_all=True, subtask_ob=False,
-                 fix_init=False, fix_init_parts=None, reset_robot_after_attach=None, control_freq=None, no_collision=False, **cfg_overrides):
+                 fix_init=False, fix_init_parts=None, reset_robot_after_attach=None, control_freq=None, no_collision=False, assembled=False,
+                 **cfg_overrides):
     """The Engine of `num_envs` envs of `agent` + `furniture_name` that both env surfaces run; `lib_path` as for Engine.  The keywords:
         `dense`: None for the sparse reward of FurnitureEnv; a dict of coefficient overrides (possibly empty) for the phase-based
         reward of FurnitureSawyerDenseRewardEnv, computed inside the step kernel (furniture_b200/dense.py).
@@ -168,11 +169,14 @@ def build_engine(agent, furniture_name, num_envs, device=0, lib_path=None, dense
         left); subtask_ob=True adds their part ids + 1 (float32).  Each env's pair follows its connections and resets inside the kernels.
         `fix_init`, `fix_init_parts`, `reset_robot_after_attach`: config/furniture.py:116-127, :169-174 (see set_reset_options).  A dense env
         takes reset_robot_after_attach from `dense`, whose phase machine follows it (None: off, or the dense reward's).
+        `assembled`: config/furniture.py:307-312, every episode starts from the welded furniture (see set_reset_options).
         `control_freq`, `no_collision`: config/furniture.py's (see set_sim_options), a value for every env or one per env.  control_freq sets
         the mj_steps of an env step (None: FeConfig.nsub, 50 = 10 Hz); it cannot be given together with an `nsub` override.
     The other keywords override FeConfig fields (default_config).  The engine records `control_type` and `resize_factor`."""
     if control_freq is not None and "nsub" in cfg_overrides:
         raise ValueError("control_freq and nsub both set the mj_steps of an env step: give one of them")
+    if agent == "Cursor" and assembled:
+        raise ValueError("assembled is built for the robot envs; the Cursor env's reset is host logic (cursor_env.FurnitureCursorEnvB200)")
     if agent == "Cursor" and (control_freq is not None or np.any(no_collision)):
         raise ValueError("the Cursor env takes its own control_freq (cursor_env.FurnitureCursorEnvB200); control_freq and no_collision "
                          "are options of the robot envs")
@@ -206,7 +210,7 @@ def build_engine(agent, furniture_name, num_envs, device=0, lib_path=None, dense
     obs_flags = dict(robot_ob=bool(robot_ob), object_ob=bool(object_ob), object_ob_all=bool(object_ob_all), subtask_ob=bool(subtask_ob))
     engine = Engine(model, num_envs, device=device, config=cfg, lib_path=lib_path, dense=dense_config(**dense) if dense is not None else None,
                     ik=ik_cfg, controller=ctl_cfg, obs_layout=obs_flags, fix_init=fix_init, fix_init_parts=fix_init_parts,
-                    reset_robot_after_attach=reset_robot_after_attach)
+                    reset_robot_after_attach=reset_robot_after_attach, assembled=assembled)
     engine.control_type, engine.resize_factor = control_type, resize_factor
     if control_freq is not None or np.any(no_collision):
         engine.set_sim_options(control_freq=control_freq, no_collision=no_collision if np.any(no_collision) else None)
@@ -257,12 +261,13 @@ class BatchedFurnitureEnv:
         """the raw bank of recorded starts that the per-env fields init_state / init_pick index (Engine.set_init_states)"""
         self.engine.set_init_states(states)
 
-    def set_reset_options(self, fix_init=None, fix_init_parts=None, reset_robot_after_attach=None, envs=None):
+    def set_reset_options(self, fix_init=None, fix_init_parts=None, reset_robot_after_attach=None, envs=None, assembled=None):
         """per env (`envs`, default: all; None leaves an option as it is): fix_init keeps the furniture's start the same in every episode (the
         XML's init poses where it lists them, else the env's first random placement; no placement draw), fix_init_parts (a set or list of part
         names, or a comma string) does so for those parts only and places the others around them, reset_robot_after_attach sends the arm back
-        to its start pose, with fresh noise, after every connection (furniture.py:916-924, :1389-1404, :1519-1532)"""
-        self.engine.set_reset_options(fix_init, fix_init_parts, reset_robot_after_attach, envs)
+        to its start pose, with fresh noise, after every connection (furniture.py:916-924, :1389-1404, :1519-1532), assembled starts every
+        episode from the welded furniture at the model's qpos0 (furniture.py:1501-1532)"""
+        self.engine.set_reset_options(fix_init, fix_init_parts, reset_robot_after_attach, envs, assembled=assembled)
 
     def set_sim_options(self, control_freq=None, no_collision=None, envs=None):
         """per env (`envs`, default: all; a scalar or one value per env of `envs`; None leaves an option as it is): control_freq sets the

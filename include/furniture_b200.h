@@ -116,7 +116,10 @@ int fe_sim_step(fe_handle* h, int nsub, void* stream);
    different counts share one launch); no_collision (int32, one per env, read/write: config/furniture.py's no_collision, furniture.py:1962-1965:
    while 1, contype = conaffinity = 0 on every geom of the agent -- every colliding geom that is neither a furniture part's nor the floor --
    through steps and resets.  Writing it changes the env's geom_contype / geom_conaffinity at once: 0 where it turns on, the model's compiled
-   masks where it turns off).  fe_set_field refuses flags outside {0, 1}, substeps below 1, fix_init_parts bits at or beyond the
+   masks where it turns off); assembled (int32, one per env, read/write: config/furniture.py:307-312.  From the env's next reset on, an
+   auto-reset included, every weld starts on with the eq_data the env holds, and a random-placement reset still draws and stores its
+   placement but leaves the parts at the model's qpos0 (their link frames), all in one group -- furniture.py:1501-1532; a recorded start
+   turns the welds on and merges no group).  fe_set_field refuses flags outside {0, 1}, substeps below 1, fix_init_parts bits at or beyond the
    number of parts, non-finite fix_pose values or zero quaternions, fix_have = 1 for an env whose fix_pose was never written and, in a dense
    handle, a reset_robot_after_attach that differs from the dense reward's */
 int fe_get_field(fe_handle* h, const char* name, void* dst_host, size_t bytes);
