@@ -73,6 +73,12 @@ struct FeEnvState {
   int* substeps;                               // [N] mj_steps of the env's step: int(control_timestep / model_timestep) (furniture.py:2878)
   int* no_collision;                           // [N] 0 / 1: the agent's masks stay 0 (config/furniture.py no_collision, furniture.py:1962-1965)
   int* assembled;                              // [N] 0 / 1: episodes start with every weld on, the parts at qpos0 (config/furniture.py:307-312)
+  // the task options of config/furniture.py per env, in fe_config's types: filled from it at creation, read instead of it by the kernels
+  double* alignment;                           // [N][4] alignment_pos_dist, _rot_dist_up, _rot_dist_forward, _project_dist (:203-226), thr[] order
+  int* auto_align;                             // [N] 0 / 1 (:95-100)
+  float* placement_rand;                       // [N][3] furn_xyz_rand, furn_rot_rand, agent_xyz_rand (:177-194)
+  float* reward_coef;                          // [N][5] success_reward, touch_reward, pick_reward, ctrl_penalty_coef, unstable_penalty_coef (:291-295)
+  int* max_episode_steps;                      // [N] (:163-168)
   int *robot_contype, *robot_conaff;           // [N][ngeom] saved robot masks during reset
   float* episode_reward;
   // dense (phase-based) reward, fe_dense.h: NULL = the sparse reward of FurnitureEnv._compute_reward
@@ -403,13 +409,13 @@ FE_FN void fe_fwd_step(FeEnv* e) { fe_substep(e->w); }
 FE_FN void fe_try_connect_scan(FeEnv* e, int part1) {
   FeWarp* w = e->w;
   const fe_scene* sc = e->sc;
-  const fe_config* cfg = e->cfg;
   LANES_BEGIN
     if (lane == 0) {
       e->si->aligned = 0;
       const int g1 = fe_find(e->group, part1);
       const int* connected = e->es.site_connected + (size_t)e->env * w->m->nsite;
-      const double thr[4] = {cfg->alignment_pos_dist, cfg->alignment_rot_dist_up, cfg->alignment_rot_dist_forward, cfg->alignment_project_dist};
+      const double* al = e->es.alignment + (size_t)e->env * 4;
+      const double thr[4] = {al[0], al[1], al[2], al[3]};
       bool found = w->m->neq > 0; // some weld joins bodies of the two candidate sets (body2_ids = every part)
       for (int i = 0; i < sc->nconn && found && !e->si->aligned; ++i) {
         if (fe_find(e->group, sc->conn_part[i]) != g1) continue;
@@ -431,7 +437,7 @@ FE_FN void fe_try_connect_scan(FeEnv* e, int part1) {
 }
 
 // _connect(site1, site2, auto_align) (furniture.py:847-924) for arm agents: the pair in si->site1 .. conn2, its target quat in sd->target_quat.
-// `align`: FE_ALIGN_CONFIG follows cfg->auto_align (a connection made by the policy); the reset's preassembly passes auto_align=_init_qpos is None
+// `align`: FE_ALIGN_CONFIG follows the env's auto_align (a connection made by the policy); the reset's preassembly passes auto_align=_init_qpos is None
 // (furniture.py:1556): FE_ALIGN_ALWAYS after random placement, FE_ALIGN_NEVER on a recorded start
 enum { FE_ALIGN_CONFIG = 0, FE_ALIGN_ALWAYS = 1, FE_ALIGN_NEVER = 2 };
 // _initialize_robot_pos (furniture.py:1761-1779), lane 0: fresh noise on every call, the arm joints at their start pose plus the noise, the
@@ -441,7 +447,7 @@ FE_HDN void fe_init_robot_pos(FeEnv* e) {
   const fe_scene* sc = e->sc;
   uint32_t* mt = e->es.mt + (size_t)e->env * FE_MT_N;
   int pos = e->es.mt_pos[e->env];
-  const double r = (double)e->cfg->agent_xyz_rand; // _init_random(shape, "agent") = rng.uniform(-r, r, size=7), furniture.py:336-349
+  const double r = (double)e->es.placement_rand[(size_t)e->env * 3 + 2]; // agent_xyz_rand; _init_random(shape, "agent") = rng.uniform(-r, r, size=7), furniture.py:336-349
   for (int i = 0; i < sc->narm; ++i) w->qpos()[sc->arm_dof[i]] = (float)ndadd((double)sc->robot_init_qpos[i], fe_mt_uniform(mt, &pos, -r, r));
   for (int i = 0; i < sc->ngrip; ++i) w->qpos()[sc->grip_dof[i]] = sc->robot_init_qpos[sc->narm + i];
   e->es.mt_pos[e->env] = pos;
@@ -462,7 +468,7 @@ FE_FN void fe_connect(FeEnv* e, int align) {
         const int gp = fe_find(e->group, p);
         if ((gp == g1 || gp == g2) && w->contype()[g] != 0) { w->contype()[g] = (1 << 30) - 1 - (1 << (g1 + 1)); w->conaff()[g] = 1 << (g1 + 1); }
       }
-      if (align == FE_ALIGN_ALWAYS || (align == FE_ALIGN_CONFIG && e->cfg->auto_align)) { // _align_connectors -> _move_site_to_target (furniture.py:1224-1250)
+      if (align == FE_ALIGN_ALWAYS || (align == FE_ALIGN_CONFIG && e->es.auto_align[e->env])) { // _align_connectors -> _move_site_to_target (furniture.py:1224-1250)
         double target[7], base[7], sp[3], sq[4];
         fe_site_pose_d(w, s1, sp, nullptr, sq);
         for (int k = 0; k < 3; ++k) target[k] = sp[k];
@@ -716,7 +722,6 @@ FE_FN void fe_env_reset_place(FeEnv* e) {
   FeWarp* w = e->w;
   const fe_model* m = w->m;
   const fe_scene* sc = e->sc;
-  const fe_config* cfg = e->cfg;
   const int nrl = m->nrlink, np = m->npart;
   LANES_BEGIN
     if (lane == 0) { // UniformRandomSampler.sample (placement_sampler.py:137-190): xy noise, z + 0.01, +furn_rot_rand deg about x
@@ -725,9 +730,10 @@ FE_FN void fe_env_reset_place(FeEnv* e) {
       const unsigned fixed = e->es.fix_init[env] && have ? (1u << np) - 1u : (have ? (unsigned)e->es.fix_init_parts[env] : 0u);
       uint32_t* mt = e->es.mt + (size_t)env * FE_MT_N;
       int pos = e->es.mt_pos[env];
-      const double half = 0.5 * (double)cfg->furn_rot_rand * 3.14159265358979323846 / 180.0;
+      const float* rnd = e->es.placement_rand + (size_t)env * 3; // furn_xyz_rand, furn_rot_rand
+      const double half = 0.5 * (double)rnd[1] * 3.14159265358979323846 / 180.0;
       const double qx[4] = {cos(half), sin(half), 0.0, 0.0};
-      const double r_xy = (double)cfg->furn_xyz_rand, r_rot = (double)cfg->furn_rot_rand;
+      const double r_xy = (double)rnd[0], r_rot = (double)rnd[1];
       double px[FE_MAXPART], py[FE_MAXPART]; // placed so far, in double like the sampler's Qpos list
       for (int p = 0; p < np; ++p) {
         const int qa = m->link_qadr[nrl + p];
@@ -938,7 +944,6 @@ FE_HD void fe_env_finish(FeEnv* e, const float* a, int act_dim, float connect, i
   FeWarp* w = e->w;
   const fe_model* m = w->m;
   const fe_scene* sc = e->sc;
-  const fe_config* cfg = e->cfg;
   const int np = m->npart, env = e->env;
   FE_SYNC;
   if (reset_now) {
@@ -975,6 +980,7 @@ FE_HD void fe_env_finish(FeEnv* e, const float* a, int act_dim, float connect, i
   // reward (furniture.py:482-541), termination (:440-445, :451-480)
   LANES_BEGIN
     if (lane == 0) {
+      const float* coef = e->es.reward_coef + (size_t)env * 5; // success, touch, pick, ctrl_penalty, unstable_penalty
       float touch_r = 0.f, pick_r = 0.f;
       int* touched = e->es.touched + (size_t)env * np;
       int* picked = e->es.picked + (size_t)env * np;
@@ -983,24 +989,25 @@ FE_HD void fe_env_finish(FeEnv* e, const float* a, int act_dim, float connect, i
           for (int p = 0; p < np; ++p) {
             const int t = w->touch()[p], both = arm == 0 ? 3 : 24;
             if ((t & both) == both) {
-              if (!touched[p]) { touched[p] = 1; touch_r += cfg->touch_reward; }
-              if (!(t & 4) && !picked[p]) { picked[p] = 1; pick_r += cfg->pick_reward; }
+              if (!touched[p]) { touched[p] = 1; touch_r += coef[1]; }
+              if (!(t & 4) && !picked[p]) { picked[p] = 1; pick_r += coef[2]; }
             }
           }
       const int nc = e->es.num_connected[env];
-      const float success_r = cfg->success_reward * (float)(nc - e->es.prev_num_connected[env]);
+      const float success_r = coef[0] * (float)(nc - e->es.prev_num_connected[env]);
       const int connected_now = e->si->aligned; // _connected: a connection was made during this step (the legs a reset preassembles are not one)
       e->es.prev_num_connected[env] = nc;
       float sq = 0.f;
       for (int k = 0; k < act_dim; ++k) sq += a[k] * a[k];
-      float reward = success_r + touch_r + pick_r - cfg->ctrl_penalty_coef * sq;
+      float reward = success_r + touch_r + pick_r - coef[3] * sq;
       const int n_goal = e->es.success_num_conn[env];
       int success = (nc == n_goal && np > 1) ? 1 : 0;
       int done = success;
       e->si->dense_pair = 0;
       if (e->es.dense) { // FurnitureSawyerEnv._step: reward, _done, info = _compute_reward(a); done = done or _done (furniture_sawyer.py:66-84)
         FeSliceWorld world = {w};
-        const double thr[4] = {cfg->alignment_pos_dist, cfg->alignment_rot_dist_up, cfg->alignment_rot_dist_forward, cfg->alignment_project_dist};
+        const double* al = e->es.alignment + (size_t)env * 4;
+        const double thr[4] = {al[0], al[1], al[2], al[3]};
         double ad[FE_MAXU + 2], dr = 0.0, di[FE_DENSE_INFO];
         for (int k = 0; k < act_dim; ++k) ad[k] = (double)a[k];
         int dd = 0;
@@ -1016,7 +1023,7 @@ FE_HD void fe_env_finish(FeEnv* e, const float* a, int act_dim, float connect, i
       }
       const int len = ++e->es.episode_len[env];
       float penalty = 0.f;
-      if (len == cfg->max_episode_steps || fail) { done = 1; if (fail) penalty = -cfg->unstable_penalty_coef; }
+      if (len == e->es.max_episode_steps[env] || fail) { done = 1; if (fail) penalty = -coef[4]; }
       reward += penalty;
       reward_out[env] = reward;
       done_out[env] = (uint8_t)done;

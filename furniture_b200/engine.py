@@ -32,6 +32,13 @@ STAT_NEWTON_SETUP, STAT_NEWTON_START, STAT_NEWTON_GRAD, STAT_NEWTON_HESSIAN, STA
 i32, f32, f64 = C.c_int32, C.c_float, C.c_double
 # the observation flags of config/furniture.py:228-258 and their defaults; other values go to fe_set_obs_layout
 OBS_DEFAULTS = dict(robot_ob=True, object_ob=True, object_ob_all=True, subtask_ob=False)
+# the task options of config/furniture.py (:95-100, :163-168, :177-194, :203-226, :291-295) -> (per-env field, column); see set_task_options
+TASK_OPTIONS = dict(
+    alignment_pos_dist=("alignment", 0), alignment_rot_dist_up=("alignment", 1), alignment_rot_dist_forward=("alignment", 2),
+    alignment_project_dist=("alignment", 3), auto_align=("auto_align", 0), furn_xyz_rand=("placement_rand", 0),
+    furn_rot_rand=("placement_rand", 1), agent_xyz_rand=("placement_rand", 2), success_reward=("reward_coef", 0),
+    touch_reward=("reward_coef", 1), pick_reward=("reward_coef", 2), ctrl_penalty_coef=("reward_coef", 3),
+    unstable_penalty_coef=("reward_coef", 4), max_episode_steps=("max_episode_steps", 0))
 
 
 class FeConfig(C.Structure):
@@ -358,6 +365,36 @@ class Engine:
             cur[idx, 0] = v
             self.set(name, cur)
 
+    def set_task_options(self, envs=None, **values):
+        """the task options of config/furniture.py for the envs in `envs` (default: all), each a scalar or one value per env of `envs`, by the
+        reference's key names (TASK_OPTIONS): the alignment thresholds and auto_align, from the env's next step; furn_xyz_rand, furn_rot_rand
+        and agent_xyz_rand, from its next reset (agent_xyz_rand also from its next connection under reset_robot_after_attach); success_reward,
+        touch_reward, pick_reward, ctrl_penalty_coef and unstable_penalty_coef, from its next step; max_episode_steps at once.  A dense handle
+        takes unstable_penalty_coef only among the coefficients: its phase machine replaces the other terms."""
+        if self.model.meta.get("agent") == "Cursor":
+            raise ValueError("the Cursor env's reward and connection logic is host code (cursor_env.FurnitureCursorEnvB200); the task options "
+                             "are options of the robot envs")
+        unknown = sorted(set(values) - set(TASK_OPTIONS))
+        if unknown:
+            raise ValueError("unknown task options %s (known: %s)" % (unknown, sorted(TASK_OPTIONS)))
+        idx = np.arange(self.N) if envs is None else np.asarray(envs, dtype=np.int64).ravel()
+        if idx.size and (idx.min() < 0 or idx.max() >= self.N):
+            raise IndexError("envs must lie in [0, %d), got %s" % (self.N, idx.tolist()))
+        fields = {}
+        for key, v in values.items():
+            if v is None:
+                continue
+            name, col = TASK_OPTIONS[key]
+            if name not in fields:
+                fields[name] = self.get(name)
+            cur = fields[name]
+            v = np.asarray(v)
+            if v.ndim > 1 or (v.ndim == 1 and v.shape != idx.shape):
+                raise ValueError("%s takes a scalar or one value per env of `envs` (%d), got shape %s" % (key, idx.size, v.shape))
+            cur[idx, col] = v.astype(cur.dtype)
+        for name, cur in fields.items():
+            self.set(name, cur)
+
     def close(self):
         if getattr(self, "h", None) and self.h.value:
             self.L.fe_destroy(self.h)
@@ -382,9 +419,9 @@ class Engine:
     _INT = {"order", "geom_contype", "geom_conaffinity", "eq_active", "touch", "flags", "ncon", "niter", "stats", "con_geom", "con_state", "group", "site_connected",
             "num_connected", "prev_num_connected", "touched", "picked", "episode_length", "done", "mt_pos", "preassembled", "num_connects",
             "init_state", "init_pick", "init_mt_pos", "subtask_part", "fix_init", "fix_init_parts", "fix_have", "reset_robot_after_attach",
-            "substeps", "no_collision", "assembled"}
+            "substeps", "no_collision", "assembled", "auto_align", "max_episode_steps"}
     _U32 = {"mt_state", "init_mt_state"}
-    _F64 = {"fix_pose"}
+    _F64 = {"fix_pose", "alignment"}
 
     def _dtype(self, name, eb):
         if eb == 8:

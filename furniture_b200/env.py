@@ -18,7 +18,7 @@ import numpy as np
 
 from . import mjcf
 from .dense import DENSE_DEFAULTS, DENSE_ENV_DEFAULTS, INFO_KEYS as DENSE_INFO_KEYS, dense_config
-from .engine import INFO_DIM, OBS_DEFAULTS, Engine, default_config
+from .engine import INFO_DIM, OBS_DEFAULTS, TASK_OPTIONS, Engine, default_config
 
 RESET_DEFAULTS = dict(fix_init=False, fix_init_parts=None, reset_robot_after_attach=False, assembled=False)  # config/furniture.py:116-127, :169-174, :307-312
 SIM_DEFAULTS = dict(control_freq=10, no_collision=False)  # config/furniture.py:71-73, :304-306
@@ -172,6 +172,9 @@ def build_engine(agent, furniture_name, num_envs, device=0, lib_path=None, dense
         `assembled`: config/furniture.py:307-312, every episode starts from the welded furniture (see set_reset_options).
         `control_freq`, `no_collision`: config/furniture.py's (see set_sim_options), a value for every env or one per env.  control_freq sets
         the mj_steps of an env step (None: FeConfig.nsub, 50 = 10 Hz); it cannot be given together with an `nsub` override.
+        The task options of config/furniture.py (TASK_OPTIONS: the alignment thresholds, auto_align, the placement noise, the reward
+        coefficients, max_episode_steps): a scalar overrides FeConfig; a sequence gives one value per env (see set_task_options), the
+        FeConfig field keeping its default.
     The other keywords override FeConfig fields (default_config).  The engine records `control_type` and `resize_factor`."""
     if control_freq is not None and "nsub" in cfg_overrides:
         raise ValueError("control_freq and nsub both set the mj_steps of an env step: give one of them")
@@ -180,6 +183,7 @@ def build_engine(agent, furniture_name, num_envs, device=0, lib_path=None, dense
     if agent == "Cursor" and (control_freq is not None or np.any(no_collision)):
         raise ValueError("the Cursor env takes its own control_freq (cursor_env.FurnitureCursorEnvB200); control_freq and no_collision "
                          "are options of the robot envs")
+    per_env = {k: cfg_overrides.pop(k) for k in list(cfg_overrides) if k in TASK_OPTIONS and np.ndim(cfg_overrides[k]) > 0}
     cfg = default_config(**cfg_overrides)
     # furn_size_rand (config/furniture.py:196-201): the reference draws one size factor per env process while loading the model.
     # A handle shares one model: the batch takes env 0's factor (the first draw of RandomState(seed)); every env's generator
@@ -214,6 +218,8 @@ def build_engine(agent, furniture_name, num_envs, device=0, lib_path=None, dense
     engine.control_type, engine.resize_factor = control_type, resize_factor
     if control_freq is not None or np.any(no_collision):
         engine.set_sim_options(control_freq=control_freq, no_collision=no_collision if np.any(no_collision) else None)
+    if per_env:
+        engine.set_task_options(**per_env)
     if prefix_length(preassembled) or num_connects is not None:
         engine.set_subtask(prefix_length(preassembled), num_connects)
     apply_init_config(engine, load_init_states, load_demo)
@@ -275,6 +281,12 @@ class BatchedFurnitureEnv:
         collision of the agent off at once (furniture.py:1962-1965), or back on with the model's masks.  Envs at different frequencies
         step together in one launch."""
         self.engine.set_sim_options(control_freq, no_collision, envs)
+
+    def set_task_options(self, envs=None, **values):
+        """per env (`envs`, default: all; a scalar or one value per env of `envs`): the alignment thresholds, auto_align, the placement
+        noise, the reward coefficients and max_episode_steps of config/furniture.py by their key names (Engine.set_task_options), so that
+        one batch can run a curriculum over them"""
+        self.engine.set_task_options(envs, **values)
 
     def set_subtask(self, subtask, num_connects=None):
         """FurnitureEnv.set_subtask (furniture.py:204-207) with a scalar or an (N,) array each, so that the envs of one batch can train different
@@ -432,6 +444,18 @@ class MixedFurnitureEnv:
             sel = (idx >= off) & (idx < off + b.num_envs)
             if sel.any():
                 b.set_sim_options(None if cf is None else cf[sel], None if nc is None else nc[sel], idx[sel] - off)
+
+    def set_task_options(self, envs=None, **values):
+        """BatchedFurnitureEnv.set_task_options with `envs` as global indices of this batch (default: all); each value is a scalar or one
+        per env of `envs`"""
+        idx = np.arange(self.real_envs) if envs is None else np.asarray(envs, dtype=np.int64).ravel()
+        if idx.size and (idx.min() < 0 or idx.max() >= self.real_envs):
+            raise IndexError("envs must lie in [0, %d), got %s" % (self.real_envs, idx.tolist()))
+        per = {k: np.broadcast_to(np.asarray(v), idx.shape) for k, v in values.items() if v is not None}
+        for b, off in zip(self.buckets, self.offsets):
+            sel = (idx >= off) & (idx < off + b.num_envs)
+            if sel.any():
+                b.set_task_options(idx[sel] - off, **{k: v[sel] for k, v in per.items()})
 
     def _obs_dict(self, obs):
         d, o = OrderedDict(), 0

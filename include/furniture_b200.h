@@ -119,9 +119,18 @@ int fe_sim_step(fe_handle* h, int nsub, void* stream);
    masks where it turns off); assembled (int32, one per env, read/write: config/furniture.py:307-312.  From the env's next reset on, an
    auto-reset included, every weld starts on with the eq_data the env holds, and a random-placement reset still draws and stores its
    placement but leaves the parts at the model's qpos0 (their link frames), all in one group -- furniture.py:1501-1532; a recorded start
-   turns the welds on and merges no group).  fe_set_field refuses flags outside {0, 1}, substeps below 1, fix_init_parts bits at or beyond the
-   number of parts, non-finite fix_pose values or zero quaternions, fix_have = 1 for an env whose fix_pose was never written and, in a dense
-   handle, a reset_robot_after_attach that differs from the dense reward's */
+   turns the welds on and merges no group); the task options of config/furniture.py, per env, read by the kernels in place of the same
+   fe_config members and set from them by fe_create: alignment (4 x float64 per env, read/write: alignment_pos_dist, alignment_rot_dist_up,
+   alignment_rot_dist_forward, alignment_project_dist, :203-226) and auto_align (int32, one per env, read/write: :95-100), from the env's next
+   step; placement_rand (3 x float32 per env, read/write: furn_xyz_rand, furn_rot_rand, agent_xyz_rand, :177-194), from the env's next reset,
+   agent_xyz_rand also from its next connection under reset_robot_after_attach; reward_coef (5 x float32 per env, read/write: success_reward,
+   touch_reward, pick_reward, ctrl_penalty_coef, unstable_penalty_coef, :291-295), from the env's next step; max_episode_steps (int32, one
+   per env, read/write: :163-168), at once, an episode ending when its length equals it (fe_set_max_episode_steps writes every env's).
+   fe_set_field refuses flags outside {0, 1}, substeps below 1, fix_init_parts bits at or beyond the
+   number of parts, non-finite fix_pose values or zero quaternions, fix_have = 1 for an env whose fix_pose was never written, non-finite
+   alignment / placement_rand / reward_coef values, max_episode_steps below 1 and, in a dense handle, a reset_robot_after_attach that
+   differs from the dense reward's or a reward_coef whose first four columns differ from the handle's fe_config (the phase machine
+   replaces those terms; its ctrl_penalty_coef is fe_dense_config's) */
 int fe_get_field(fe_handle* h, const char* name, void* dst_host, size_t bytes);
 int fe_set_field(fe_handle* h, const char* name, const void* src_host, size_t bytes);
 int fe_field_dim(fe_handle* h, const char* name, int* dim, int* elem_bytes);
@@ -194,7 +203,7 @@ int fe_env_step_packed(fe_handle* h, const float* actions_dev, float* packed_dev
 /* same call with host buffers: H2D of the actions and D2H of the results happen inside (pinned staging) */
 int fe_env_step_host(fe_handle* h, const float* actions_host, float* obs_host, float* reward_host, uint8_t* done_host, int32_t* info_host);
 /* FurnitureGym.set_max_episode_steps -> FurnitureEnv.set_max_episode_steps (furniture_gym.py:35-37, furniture.py:271-272):
-   takes effect from the next step */
+   every env's field max_episode_steps and the handle's fe_config; takes effect from the next step */
 int fe_set_max_episode_steps(fe_handle* h, int max_episode_steps);
 /* Switch the handle to the dense reward; call before the first fe_env_reset.  The scene must carry a recipe, and dc->phase_ob must agree
  * with the scene (the one-hot phase is part of obs_dim).  fe_env_step then returns the dense reward / done / success, and field
