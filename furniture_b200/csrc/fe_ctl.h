@@ -173,13 +173,15 @@ FE_HDN void fe_ctl_torques(const fe_ctl_config* c, FeCtlState* s, const double* 
   }
 }
 
-// test hook: one thread walks the records of one episode (a record with reset != 0 starts with a fresh controller)
+// test hook: one thread walks the records of one episode; reset byte 1 starts a fresh controller, 2 calls Controller.reset() on the existing
+// one (what FurnitureEnv._reset does between episodes: ori_set survives)
 FE_HDN void fe_ctl_eval_episode(const fe_ctl_config* c, int first, int count, const uint8_t* reset, const uint8_t* policy_step, const double* action /* [7] per record */,
                                 const FeCtlIn* in, double* tau /* [7] per record */) {
   FeCtlState s;
   s.ori_set = 0; s.started = 0;
   for (int t = first; t < first + count; ++t) {
-    if (reset[t]) { s.ori_set = 0; fe_ctl_reset(c, &s); }
+    if (reset[t] == 1) s.ori_set = 0;
+    if (reset[t]) fe_ctl_reset(c, &s);
     fe_ctl_torques(c, &s, action + (size_t)7 * t, policy_step[t], in + t, tau + (size_t)7 * t);
   }
 }

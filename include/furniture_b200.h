@@ -282,7 +282,9 @@ typedef struct fe_ctl_config {
 int fe_enable_controller(fe_handle* h, const fe_ctl_config* cc);
 /* test hook: the device controller arithmetic on explicit simulator readings.  Records [first[e], first[e] + count[e]) form episode e; per
  * record: reset / policy_step flags, action (7 doubles, the first control_dim used) and the readings as 123 doubles: pos 3, R 9 (row-major),
- * velp 3, velr 3, q 7, qvel 7, Jx 21, Jr 21 (3 x 7 row-major), M 49.  Output: torques (7 doubles per record). */
+ * velp 3, velr 3, q 7, qvel 7, Jx 21, Jr 21 (3 x 7 row-major), M 49.  Output: torques (7 doubles per record).
+ * reset byte: 0 carries the controller on; 1 starts a new controller (nothing carried over); 2 calls Controller.reset() on the existing one, as
+ * FurnitureEnv._reset does between episodes (the position controller keeps the orientation goal of its first policy step). */
 int fe_ctl_eval(fe_handle* h, const fe_ctl_config* cc, int n_episodes, const int32_t* first, const int32_t* count, int n_records, const uint8_t* reset,
                 const uint8_t* policy_step, const double* action, const double* readings, double* torques_host);
 

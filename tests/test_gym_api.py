@@ -1,7 +1,8 @@
-"""Single-env gym surface (FurnitureGym, furniture_gym.py:11-80) over the engine, on the lane-emulated build: observation dict
+"""Single-env gym surface (FurnitureGym, furniture_gym.py:11-80) over the engine, on the lane-emulated build (the torque controllers on the CUDA build too): observation dict
 layout, reward / done as Python scalars, the reference's episode keys in `info` at episode end, and one reset's worth of numpy
 draws per episode (the env equals the oracle env seeded the same way across an episode boundary)."""
 import numpy as np
+import pytest
 
 from furniture_b200.gym_api import FurnitureGymB200
 from oracle.ref_env import Cfg, OracleFurnitureEnv
@@ -182,8 +183,19 @@ def test_ik_control_type_through_the_gym_surface():
 def test_torque_controllers_through_the_gym_surface():
     """control_type in NEW_CONTROLLERS (furniture.py:41-47): the scene switches to the torque-actuated Sawyer, the action is the controller's
     command + gripper + connect, robot_ob the 15-number proprioception of every non-impedance control type (furniture_sawyer.py:110-155)"""
+    _torque_controllers_through_the_gym_surface(False)
+
+
+@pytest.mark.gpu
+def test_torque_controllers_through_the_gym_surface_cuda():
+    """the same on the CUDA build"""
+    _torque_controllers_through_the_gym_surface(True)
+
+
+def _torque_controllers_through_the_gym_surface(gpu):
+    lib = dict(device=0) if gpu else dict(lib_path=build_emu())
     for ct, dof in (("position_orientation", 8), ("position", 5), ("joint_impedance", 9), ("joint_velocity", 9), ("joint_torque", 9)):
-        env = FurnitureGymB200(name="FurnitureSawyerEnv", lib_path=build_emu(), control_type=ct, nsub=3, max_episode_steps=2, move_speed=0.05)
+        env = FurnitureGymB200(name="FurnitureSawyerEnv", control_type=ct, nsub=3, max_episode_steps=2, move_speed=0.05, **lib)
         assert env.dof == dof and env.model.meta["agent"] == "SawyerTorque" and abs(env.ctl_cfg.move_speed - 0.05) < 1e-12
         ob = env.reset()
         assert ob["robot_ob"].shape == (15,)

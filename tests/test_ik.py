@@ -110,7 +110,7 @@ def _ik_state(eng, i):
                 s2=f[4:8], target_pos2=f[11:14], q_cmd2=f[21:28], low_all=f[28:44], iters2=int(it[1]))
 
 
-QUAT_BACKENDS = BACKENDS + [pytest.param("emu-quaternion", id="emu-ik_quaternion")]  # the quaternion variant: lane-emulated build only
+QUAT_BACKENDS = BACKENDS + [pytest.param("emu-quaternion", id="emu-ik_quaternion"), pytest.param("cuda-quaternion", id="cuda-ik_quaternion", marks=pytest.mark.gpu)]
 
 
 @pytest.mark.parametrize("gpu", QUAT_BACKENDS)
@@ -122,8 +122,9 @@ def test_ik_env_steps_match_the_cpu_env(sawyer, gpu):
 
     m = sawyer
     n = 2
-    quat = gpu == "emu-quaternion"
-    gpu = False if quat else gpu
+    quat = gpu in ("emu-quaternion", "cuda-quaternion")
+    if quat:
+        gpu = gpu == "cuda-quaternion"
     eng = _ik_engine(m, n, gpu, quaternion_mode=int(quat))
     dof = 9 if quat else 8
     assert eng.act_dim == dof
@@ -224,6 +225,16 @@ def test_enable_ik_and_dense_refuse_what_they_cannot_serve(sawyer):
 def test_dense_reward_under_ik_control_matches_the_cpu_env(sawyer):
     """IKEASawyerDense-v0 with the reference's default control type: the phase machine reads the policy's 8-number action (gripper = ac[-2],
     connect = ac[-1], control penalty on ac[:-2]) while the arm is driven by the IK's joint velocities -- device vs CPU env, emulated build"""
+    _dense_reward_under_ik_control(sawyer, False)
+
+
+@pytest.mark.gpu
+def test_dense_reward_under_ik_control_matches_the_cpu_env_cuda(sawyer):
+    """the same on the CUDA build"""
+    _dense_reward_under_ik_control(sawyer, True)
+
+
+def _dense_reward_under_ik_control(sawyer, gpu):
     from furniture_b200.dense import dense_config
     from furniture_b200.engine import Engine, default_config
     from oracle.ref_env import DenseCfg, OracleDenseIKEnv
@@ -232,7 +243,9 @@ def test_dense_reward_under_ik_control_matches_the_cpu_env(sawyer):
     from test_env_parity import _sync_oracle_from_engine
 
     m = sawyer
-    eng = Engine(m, 1, config=default_config(**DENSE_BASE), lib_path=build_emu(), dense=dense_config(), ik=IK.ik_config(m))
+    c = default_config(**DENSE_BASE)
+    eng = (Engine(m, 1, device=0, config=c, dense=dense_config(), ik=IK.ik_config(m)) if gpu
+           else Engine(m, 1, config=c, lib_path=build_emu(), dense=dense_config(), ik=IK.ik_config(m)))
     eng.env_reset()
     e = OracleDenseIKEnv(m, DenseCfg())
     e.reset()
@@ -265,11 +278,21 @@ def test_dense_reward_under_ik_control_matches_the_cpu_env(sawyer):
 def test_unstable_ik_step_resets_mid_step_and_once_more_at_the_end(sawyer):
     """a _do_simulation that blows up inside _do_ik_step resets the env on the spot and the remaining repeats run on the new episode
     (furniture.py:2889-2897 inside the loop of :2977-2995); the step then ends the episode with the unstable penalty and the VecEnv worker
-    resets again: three resets' worth of random draws in all, like the impedance path"""
+    resets again: three resets' worth of random draws in all, like the impedance path -- emulated build"""
+    _unstable_ik_step(sawyer, False)
+
+
+@pytest.mark.gpu
+def test_unstable_ik_step_resets_mid_step_and_once_more_at_the_end_cuda(sawyer):
+    """the same on the CUDA build"""
+    _unstable_ik_step(sawyer, True)
+
+
+def _unstable_ik_step(sawyer, gpu):
     from oracle.ref_env import Cfg, OracleFurnitureEnv
 
     m, seed = sawyer, 99
-    eng = _ik_engine(m, 2, False, seed=seed, nsub=2)
+    eng = _ik_engine(m, 2, gpu, seed=seed, nsub=2)
     eng.env_reset()
     v = eng.get("qvel").copy()
     v[1, 0] = 1e8
@@ -296,10 +319,11 @@ def test_unstable_ik_step_resets_mid_step_and_once_more_at_the_end(sawyer):
     assert np.isfinite(eng.get("ik_state")[1].view(np.float32)[:44]).all()  # the new episode's targets were re-synchronised from a sane pose
 
 
-@pytest.mark.parametrize("quat", [0, 1], ids=["ik", "ik_quaternion"])
-def test_baxter_ik_env_steps_match_the_cpu_env(quat):
+@pytest.mark.parametrize("gpu,quat", [pytest.param(False, 0, id="ik"), pytest.param(False, 1, id="ik_quaternion"),
+                                      pytest.param(True, 0, id="cuda-ik", marks=pytest.mark.gpu), pytest.param(True, 1, id="cuda-ik_quaternion", marks=pytest.mark.gpu)])
+def test_baxter_ik_env_steps_match_the_cpu_env(gpu, quat):
     """control_type="ik" / "ik_quaternion" on the two-arm env (15 / 17-number actions: move / rotate per arm, two grippers, connect): both
-    arms' targets, joint commands and low-level actions, observation and reward of the device equal the CPU env -- emulated build"""
+    arms' targets, joint commands and low-level actions, observation and reward of the device equal the CPU env"""
     from furniture_b200.engine import Engine, default_config
     from oracle.ref_env import OracleIKEnv
     from parity_util import build_emu
@@ -308,7 +332,7 @@ def test_baxter_ik_env_steps_match_the_cpu_env(quat):
     m = mjcf.load_scene("Baxter", "chair_ingolf_0650")
     ikc = IK.ik_config(m, quaternion_mode=quat)
     assert ikc.narms == 2 and abs(ikc.kp - 2.0) < 1e-9 and abs(ikc.user_sensitivity - 1.0) < 1e-9 and abs(ikc.damping - 0.7) < 1e-7
-    eng = Engine(m, 1, config=default_config(), lib_path=build_emu(), ik=ikc)
+    eng = Engine(m, 1, device=0, config=default_config(), ik=ikc) if gpu else Engine(m, 1, config=default_config(), lib_path=build_emu(), ik=ikc)
     dof = 17 if quat else 15
     assert eng.act_dim == dof
     eng.env_reset()

@@ -169,8 +169,7 @@ def test_env_step_matches_cpu_env(sawyer_model, gpu, kind, control_freq, no_coll
 
 # ------------------------------------------------------------------ one handle, mixed values
 @pytest.mark.parametrize("gpu,control_type", [pytest.param(g, c, id="%s-%s" % ("cuda" if g else "emu", c), marks=[pytest.mark.gpu] if g else [])
-                                                for g in (False, True) for c in ("impedance", "ik")]
-                         + [pytest.param(False, "position", id="emu-position")])  # the controller step's CUDA path has not run on a GPU
+                                                for g in (False, True) for c in ("impedance", "ik", "position")])
 def test_mixed_frequencies_equal_uniform_handles(gpu, control_type):
     """envs at 10 / 20 / 5 / 10 Hz in one handle equal, bit for bit, the same envs of handles that run one frequency for all their envs,
     over reset + 5 steps with an auto-reset (max_episode_steps 3).  On the GPU the first step runs on the initial packing, envs 16 b ..
