@@ -37,15 +37,25 @@ def make_engine(model, n_envs, use_gpu, **cfg):
     return Engine(model, n_envs, config=c, lib_path=build_emu())
 
 
+def joint_qadr(model, names):
+    """qpos addresses of the named (hinge / slide) joints"""
+    return np.array([model.jnt_qposadr[model.names["jnt"].index(n)] for n in names], dtype=np.int64)
+
+
+def arm_qadr(model):
+    """qpos addresses of the agent's arm joints and of its gripper joints, in the order of robot_init_qpos /
+    gripper_init_qpos (Baxter: the head pan is dof 0 and every arm has its gripper after it, so neither set is contiguous)"""
+    return joint_qadr(model, model.meta["robot_joints"]), joint_qadr(model, model.meta["gripper_joints"])
+
+
 def settled_state(model, seed=0, robot_noise=0.3, dz=0.01):
     """qpos with parts at their XML init poses (+dz) and the arm near its init pose."""
     rng = np.random.RandomState(seed)
     q = model.qpos0.copy()
     meta = model.meta
-    nr = len(meta["robot_init_qpos"])
-    ng = len(meta["gripper_init_qpos"])
-    q[:nr] = meta["robot_init_qpos"] + rng.uniform(-robot_noise, robot_noise, nr)
-    q[nr : nr + ng] = meta["gripper_init_qpos"]
+    arm, grip = arm_qadr(model)
+    q[arm] = meta["robot_init_qpos"] + rng.uniform(-robot_noise, robot_noise, len(arm))
+    q[grip] = meta["gripper_init_qpos"]
     for name in meta["part_names"]:
         qa = model.jnt_qposadr[model.names["jnt"].index(name)]
         if name in meta["part_init_qpos"]:

@@ -11,33 +11,74 @@ import pytest
 from furniture_b200 import mjcf
 from furniture_b200.engine import STAT_COUPLED, STAT_NEWTON_SOLVES
 from oracle.oracle import OracleSim
-from parity_util import have_gpu, make_engine, oracle_link_poses, quat_err, settled_state, to_z
+from test_solver_branches import _mpr
+from parity_util import arm_qadr, have_gpu, make_engine, oracle_link_poses, quat_err, settled_state, to_z
 
 BACKENDS = [pytest.param(False, id="emu"), pytest.param(True, id="cuda", marks=pytest.mark.gpu)]
 G = os.path.join(os.path.dirname(__file__), "golden")
 
 
 def _pose_arm_over_parts(model, sim_q, rng):
-    """random arm poses that often bring links / fingers into contact with parts and floor"""
+    """random arm poses that often bring links / fingers into contact with parts and floor; the fingers anywhere in their range"""
     q = sim_q.copy()
-    q[:7] = model.meta["robot_init_qpos"] + rng.uniform(-0.8, 0.8, 7)
-    q[7:9] = rng.uniform([-0.0115, -0.020833], [0.020833, 0.0115])
+    arm, grip = arm_qadr(model)
+    q[arm] = model.meta["robot_init_qpos"] + rng.uniform(-0.8, 0.8, len(arm))
+    lo, hi = _joint_ranges(model, model.meta["gripper_joints"])
+    q[grip] = rng.uniform(lo, hi)
     return q
 
 
+def _joint_ranges(model, names):
+    r = np.array([model.a["jnt_range"][model.names["jnt"].index(n)] for n in names], dtype=np.float64)
+    return r[:, 0], r[:, 1]
+
+
+def _actuator_force(model, u, q, v):
+    """MuJoCo's actuator force before its force clamp (gain * clamped ctrl + bias), per actuator, for the host-side checks"""
+    lo, hi = model.actuator_ctrlrange[:, 0], model.actuator_ctrlrange[:, 1]
+    lim = np.asarray(model.a["actuator_ctrllimited"]).astype(bool)
+    c = np.where(lim, np.clip(u, lo, hi), u)
+    jq = model.jnt_qposadr[np.asarray(model.a["actuator_jntid"])]
+    jd = np.asarray(model.a["jnt_dofadr"])[np.asarray(model.a["actuator_jntid"])]
+    gain = np.asarray(model.a["actuator_gainprm"]).reshape(model.nu, -1)[:, 0]
+    bias = np.asarray(model.a["actuator_biasprm"]).reshape(model.nu, -1)[:, :3]
+    gear = np.asarray(model.a["actuator_gear"]).reshape(model.nu, -1)[:, 0]
+    return gain * c + bias[:, 0] + bias[:, 1] * gear * q[jq] + bias[:, 2] * gear * v[jd]
+
+
+# every arm agent, with its own tree: Sawyer (9 dofs, a chain), SawyerTorque (motor actuators), Baxter (19 dofs: the head pan,
+# two arms as separate branches, armature on 15 dofs, 1 mm contact margins, fe_robot_solve_regs<24>)
+ARM_SCENES = [pytest.param("Sawyer", "table_lack_0825", id="Sawyer"), pytest.param("SawyerTorque", "table_lack_0825", id="SawyerTorque"),
+              pytest.param("Baxter", "chair_ingolf_0650", id="Baxter")]
+
+
 @pytest.mark.parametrize("gpu", BACKENDS)
-def test_forward_stages_match_oracle(sawyer_model, gpu):
-    m = sawyer_model
+@pytest.mark.parametrize("agent,furn", ARM_SCENES)
+def test_forward_stages_match_oracle(agent, furn, gpu):
+    m = mjcf.load_scene(agent, furn)
     n = 16
     eng = make_engine(m, n, gpu)
     em = eng.em
+    nr = em.nrlink
     rng = np.random.RandomState(7)
     Q, V, U = [], [], []
     for i in range(n):
         q = settled_state(m, i, robot_noise=0.3, dz=rng.uniform(-0.003, 0.01))
         if i % 2:
             q = _pose_arm_over_parts(m, q, rng)
-        Q.append(q); V.append(rng.normal(size=m.nv) * 0.3); U.append(rng.uniform(-1.5, 1.5, m.nu))
+        v = rng.normal(size=m.nv) * 0.3
+        u = rng.uniform(-1.5, 1.5, m.nu)
+        if agent == "SawyerTorque":
+            u *= m.actuator_ctrlrange[:, 1]  # motor torques over 1.5 x their range
+        Q.append(q); V.append(v); U.append(u)
+    # the case set does reach both clamps of fe_kin_smooth: controls outside ctrlrange, and position-servo fingers whose
+    # force (gain 1e4) is past their forcerange
+    lo, hi = m.actuator_ctrlrange[:, 0], m.actuator_ctrlrange[:, 1]
+    assert sum(((u < lo) | (u > hi)).sum() for u in U) >= n
+    fl = np.asarray(m.a["actuator_forcelimited"]).astype(bool)
+    flo, fhi = np.asarray(m.a["actuator_forcerange"]).reshape(m.nu, 2).T
+    af = np.array([_actuator_force(m, u, q, v) for u, q, v in zip(U, Q, V)])[:, fl]
+    assert ((af < flo[fl]) | (af > fhi[fl])).sum() >= n and ((af > flo[fl]) & (af < fhi[fl])).any()
     eng.set("qpos", np.array(Q)); eng.set("qvel", np.array(V)); eng.set("ctrl", np.array(U))
     eng.forward()
     lp, lq = eng.get("link_xpos"), eng.get("link_xquat")
@@ -54,10 +95,10 @@ def test_forward_stages_match_oracle(sawyer_model, gpu):
         xp, xq, xm = oracle_link_poses(sim, em)
         assert np.abs(lp[i].reshape(-1, 3) - xp).max() < 1e-6                      # positions, metres
         assert max(quat_err(a, b) for a, b in zip(lq[i].reshape(-1, 4), xq)) < 1e-6
-        M = sim.qM.reshape(m.nv, m.nv)[:9, :9]
-        assert np.abs(Mr[i].reshape(9, 9) - M).max() < 1e-5 * np.abs(M).max()       # CRBA
-        assert np.abs(bias[i] - sim.qfrc_bias[:9]).max() < 1e-4 * max(1, np.abs(sim.qfrc_bias[:9]).max())  # RNE
-        assert np.abs(fs[i][:9] - sim.qfrc_smooth[:9]).max() < 1e-4 * max(1, np.abs(sim.qfrc_smooth[:9]).max())
+        M = sim.qM.reshape(m.nv, m.nv)[:nr, :nr]
+        assert np.abs(Mr[i].reshape(nr, nr) - M).max() < 1e-5 * np.abs(M).max()       # CRBA
+        assert np.abs(bias[i] - sim.qfrc_bias[:nr]).max() < 1e-4 * max(1, np.abs(sim.qfrc_bias[:nr]).max())  # RNE
+        assert np.abs(fs[i][:nr] - sim.qfrc_smooth[:nr]).max() < 1e-4 * max(1, np.abs(sim.qfrc_smooth[:nr]).max())
         zs = to_z(m, em, xm, sim.qacc_smooth)
         assert np.abs(as_[i] - zs).max() < 2e-4 * max(1, np.abs(zs).max())
         assert flags[i] == 0
@@ -67,9 +108,9 @@ def test_forward_stages_match_oracle(sawyer_model, gpu):
         total_con += len(oc)
         any_mpr = False
         for c, o in enumerate(oc):
-            # analytic pairs agree to fp32 round-off; MPR pairs (cylinder vs sphere/cylinder/box) stop at the portal
+            # analytic pairs agree to fp32 round-off; MPR pairs (a cylinder or capsule off the plane, a mesh) stop at the portal
             # tolerance 1e-6 of the Minkowski difference, which bounds depth to ~1e-5 and the normal to ~1e-3
-            mpr = 5 in (m.geom_type[o.geom1], m.geom_type[o.geom2]) and 0 not in (m.geom_type[o.geom1], m.geom_type[o.geom2])
+            mpr = _mpr(m, [o])
             any_mpr |= bool(mpr)
             assert abs(cdist[i][c] - o.dist) < (1e-4 if mpr else 2e-6), (i, c, cdist[i][c], o.dist)
             assert np.abs(cpos[i].reshape(-1, 3)[c] - np.array(list(o.pos))).max() < (2e-3 if mpr else 5e-6)
@@ -85,13 +126,13 @@ def test_forward_stages_match_oracle(sawyer_model, gpu):
         if not any_mpr:
             assert np.abs(x[i] - zo).max() < 2e-3 * max(1.0, np.abs(zo).max()), (i, np.abs(x[i] - zo).max(), np.abs(zo).max())
         Mx = np.zeros(m.nv)
-        Mx[:9] = Mr[i].reshape(9, 9).astype(np.float64) @ x[i][:9]
+        Mx[:nr] = Mr[i].reshape(nr, nr).astype(np.float64) @ x[i][:nr]
         for p in range(em.npart):
-            I = linert[i].reshape(-1, 10)[9 + p].astype(np.float64)
+            I = linert[i].reshape(-1, 10)[nr + p].astype(np.float64)
             mass, h, Io = I[0], I[1:4], np.array([[I[4], I[7], I[8]], [I[7], I[5], I[9]], [I[8], I[9], I[6]]])
-            w_, v_ = x[i][9 + 6 * p : 12 + 6 * p].astype(np.float64), x[i][12 + 6 * p : 15 + 6 * p].astype(np.float64)
-            Mx[9 + 6 * p : 12 + 6 * p] = Io @ w_ + np.cross(h, v_)
-            Mx[12 + 6 * p : 15 + 6 * p] = mass * v_ - np.cross(h, w_)
+            w_, v_ = x[i][nr + 6 * p : nr + 6 * p + 3].astype(np.float64), x[i][nr + 6 * p + 3 : nr + 6 * p + 6].astype(np.float64)
+            Mx[nr + 6 * p : nr + 6 * p + 3] = Io @ w_ + np.cross(h, v_)
+            Mx[nr + 6 * p + 3 : nr + 6 * p + 6] = mass * v_ - np.cross(h, w_)
         res = Mx - fs[i] - fc[i]
         assert np.abs(res).max() < 2e-4 * max(1.0, np.abs(fs[i]).max(), np.abs(fc[i]).max()), (i, np.abs(res).max())
     assert total_con > 100  # the cases do exercise contact
