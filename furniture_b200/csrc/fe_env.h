@@ -49,6 +49,9 @@ typedef struct fe_scene {
 
 struct FeEnvState {
   float* obs;                                  // [N][obs_dim]
+  // the last observation row and qpos / qvel of the episode an env's step ended, written by that step before its auto-reset; the rows of
+  // envs whose step did not end an episode are left as they are
+  float *terminal_obs, *terminal_qpos, *terminal_qvel; // [N][obs_dim], [N][nq], [N][nv]
   float* packed;                               // optional second output of a step: rows [obs | reward | done] (float), stride obs_dim + 2 --
                                                // the send buffer of the multi-GPU all-gather, written by the step kernel itself
   int *group, *site_connected;                 // [N][npart], [N][nsite]
@@ -302,13 +305,13 @@ struct FeEnv {
   FeWarp* w;      // header of the env's slice
   const fe_scene* sc;
   const fe_config* cfg;
-  FeState st;
-  FeEnvState es;
   int env;
-  // smem-resident env scratch
+  // smem-resident env scratch, ahead of the two state structs so that their size does not move it
   int* group;     // [npart] union-find parents (furniture.py:2738-2759)
   FeEnvScratchI* si;
   FeEnvScratchD* sd;
+  FeState st;
+  FeEnvState es;
 };
 
 FE_HD int fe_find(int* g, int i) { while (g[i] != i) i = g[i]; return i; } // path compression does not change results
@@ -583,8 +586,9 @@ FE_HD void fe_write_robot_ob(FeEnv* e, float* rb, int lane) {
 }
 
 // _get_obs under the flags of fe_set_obs_layout (furniture.py:1344-1387): the row [object_ob | subtask_ob | robot_ob | phase_ob], each entry present
-// as its flag asks.  It shows the subtask pair held in subtask_part, which the step's dense reward has not moved yet.
-FE_FN void fe_write_obs_layout(FeEnv* e) {
+// as its flag asks, written to `ob` and, when `packed` is set, to that second row too.  It shows the subtask pair held in subtask_part, which the
+// step's dense reward has not moved yet.
+FE_FN void fe_write_obs_layout(FeEnv* e, float* ob, float* packed) {
   FeWarp* w = e->w;
   const fe_model* m = w->m;
   const fe_scene* sc = e->sc;
@@ -592,9 +596,8 @@ FE_FN void fe_write_obs_layout(FeEnv* e) {
   const int* pair = e->es.subtask_part + 2 * e->env;
   const bool all = !(lay & (FE_OBS_NO_OBJECT | FE_OBS_PAIR_ONLY)), two = (lay & (FE_OBS_NO_OBJECT | FE_OBS_PAIR_ONLY)) == FE_OBS_PAIR_ONLY;
   const int nobj = all ? 7 * np : (two ? 14 : 0), nsub = (lay & FE_OBS_SUBTASK) ? 2 : 0;
-  float* ob = e->es.obs + (size_t)e->env * sc->obs_dim;
-  for (int pass = 0; pass < (e->es.packed ? 2 : 1); ++pass) {
-  if (pass == 1) ob = e->es.packed + (size_t)e->env * (sc->obs_dim + 2);
+  for (int pass = 0; pass < (packed ? 2 : 1); ++pass) {
+  if (pass == 1) ob = packed;
   LANES_BEGIN
     const int p1 = pair[0], p2 = pair[1];
     if (all) {
@@ -613,17 +616,16 @@ FE_FN void fe_write_obs_layout(FeEnv* e) {
   }
 }
 
-// _get_obs: object_ob (7 per part, XML order) then robot_ob (furniture.py:1344-1387, furniture_sawyer.py:103-155); the other flags' rows are
-// fe_write_obs_layout's
-FE_FN void fe_write_obs(FeEnv* e) {
+// _get_obs: object_ob (7 per part, XML order) then robot_ob (furniture.py:1344-1387, furniture_sawyer.py:103-155), into the row `ob` and, when
+// `packed` is set, into that second row too; the other flags' rows are fe_write_obs_layout's
+FE_FN void fe_write_obs(FeEnv* e, float* ob, float* packed) {
   FeWarp* w = e->w;
   const fe_model* m = w->m;
   const fe_scene* sc = e->sc;
-  if (sc->obs_layout) { fe_write_obs_layout(e); return; }
-  float* ob = e->es.obs + (size_t)e->env * sc->obs_dim;
+  if (sc->obs_layout) { fe_write_obs_layout(e, ob, packed); return; }
   const int nrl = m->nrlink, np = m->npart;
-  for (int pass = 0; pass < (e->es.packed ? 2 : 1); ++pass) {
-  if (pass == 1) ob = e->es.packed + (size_t)e->env * (sc->obs_dim + 2);
+  for (int pass = 0; pass < (packed ? 2 : 1); ++pass) {
+  if (pass == 1) ob = packed;
   LANES_BEGIN
     for (int p = lane; p < np; p += 32) {
       for (int k = 0; k < 3; ++k) ob[7 * p + k] = w->lpos()[3 * (nrl + p) + k];
@@ -633,6 +635,25 @@ FE_FN void fe_write_obs(FeEnv* e) {
     if (sc->phase_ob && lane < 8) ob[sc->obs_dim - 8 + lane] = (e->es.dstate && e->es.dstate[e->env].phase == lane) ? 1.f : 0.f;
   LANES_END
   }
+}
+// the env's rows of the step's outputs: obs, and the packed [obs | reward | done] row of fe_env_step_packed when it runs
+FE_HD void fe_write_step_obs(FeEnv* e) {
+  const int od = e->sc->obs_dim;
+  fe_write_obs(e, e->es.obs + (size_t)e->env * od, e->es.packed ? e->es.packed + (size_t)e->env * (od + 2) : nullptr);
+}
+// the episode that ends in this step, before the auto-reset overwrites the slice: its last observation row (the row fe_write_step_obs would
+// have written) into terminal_obs, its qpos / qvel into terminal_qpos / terminal_qvel
+FE_FN void fe_write_terminal(FeEnv* e) {
+  FeWarp* w = e->w;
+  const fe_model* m = w->m;
+  const size_t env = (size_t)e->env;
+  fe_write_obs(e, e->es.terminal_obs + env * e->sc->obs_dim, nullptr);
+  float* q = e->es.terminal_qpos + env * m->nq;
+  float* v = e->es.terminal_qvel + env * m->nv;
+  LANES_BEGIN
+    for (int i = lane; i < m->nq; i += 32) q[i] = w->qpos()[i];
+    for (int i = lane; i < m->nv; i += 32) v[i] = w->qvel()[i];
+  LANES_END
 }
 
 // stabilise furniture: 10 x { stop(gravity=0); 10 x { forward; step; slow } }  (furniture.py:1535-1540, :1560-1566)
@@ -834,7 +855,7 @@ FE_FN void fe_env_reset_sync(FeEnv* e, int pre) {
       }
     }
   LANES_END
-  fe_write_obs(e);
+  fe_write_step_obs(e);
 }
 // set_env_state(_init_qpos) (furniture.py:1794-1798) from bank entry s: _stop_objects(gravity=0), qpos and qvel, ctrl = 0.  `robot`: the first call
 // of the reset, which switches the robot's collisions back on (:1505-1517)
@@ -1039,9 +1060,12 @@ FE_HD void fe_env_finish(FeEnv* e, const float* a, int act_dim, float connect, i
     }
   LANES_END
   if (e->si->done) {
+    // The finished episode's last observation and state, taken between the two resets of an unstable step: after the one of _do_simulation's
+    // except branch, whose freshly reset world is what the reference's step returns (furniture.py:2889-2897), and before the auto-reset
+    fe_write_terminal(e);
     fe_env_reset_one(e);
   } else {
-    fe_write_obs(e);
+    fe_write_step_obs(e);
     // FurnitureSawyerEnv._step takes the observation before _compute_reward (furniture_sawyer.py:66-84): it shows the pair as the connect scan
     // left it, and the dense reward's new subtask pair is the env's from here on
     LANES_BEGIN if (lane == 0 && e->si->dense_pair) fe_dense_subtask_pair(e, e->es.dstate[env].subtask); LANES_END

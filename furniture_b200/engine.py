@@ -257,8 +257,9 @@ class Engine:
         L.fe_last_error.argtypes = [C.c_void_p]
         for f in ("fe_model_sizeof", "fe_scene_sizeof", "fe_config_sizeof"):
             getattr(L, f).restype = C.c_size_t
-        L.fe_obs_dev.restype = C.c_void_p
-        L.fe_obs_dev.argtypes = [C.c_void_p]
+        for f in ("fe_obs_dev", "fe_terminal_obs_dev", "fe_terminal_qpos_dev", "fe_terminal_qvel_dev"):
+            getattr(L, f).restype = C.c_void_p
+            getattr(L, f).argtypes = [C.c_void_p]
         self.is_cuda = bool(L.fe_is_cuda())
         if lib_path is None and not self.is_cuda:
             raise RuntimeError("furniture_b200: default library is not a CUDA build")
@@ -630,6 +631,21 @@ class Engine:
 
     def obs_dev_ptr(self):
         return self.L.fe_obs_dev(self.h)
+
+    # ---- what a finished episode left (the terminal `ob` of FurnitureEnv.step, furniture.py:364-385): the step that returns done = 1 for an
+    # env writes its last observation row and qpos / qvel before the auto-reset; other envs' rows keep what they held
+    def terminal_obs(self):
+        """(N, obs_dim) float32 host copy of the terminal observation rows, valid where the last step's done is 1"""
+        return self.get("terminal_obs")
+
+    def terminal_state(self):
+        """(qpos (N, nq), qvel (N, nv)) float32 host copies of the terminal state, valid where the last step's done is 1"""
+        return self.get("terminal_qpos"), self.get("terminal_qvel")
+
+    def terminal_dev_ptrs(self):
+        """device pointers of the terminal buffers: (obs (N, obs_dim), qpos (N, nq), qvel (N, nv)), float32, env-major; the obs pointer moves
+        with set_obs_layout"""
+        return self.L.fe_terminal_obs_dev(self.h), self.L.fe_terminal_qpos_dev(self.h), self.L.fe_terminal_qvel_dev(self.h)
 
     def is_aligned(self, p1, m1, p2, m2, angles, nangles, thr):
         n = len(p1)

@@ -40,6 +40,17 @@ FURNITURE_NAMES = (
     "three_blocks three_blocks_peg toy_table toy_table_flip tvunit_0406 tvunit_lack_0829 tvunit_lack_0830").split()
 
 
+def device_view(ptr, shape, device):
+    """a float32 torch tensor over `shape` contiguous floats of device memory at `ptr` that the engine owns (no copy; valid while the
+    engine lives)"""
+    import torch
+
+    class _Buf:
+        __cuda_array_interface__ = dict(shape=tuple(int(n) for n in shape), typestr="<f4", data=(int(ptr), False), version=2, strides=None)
+
+    return torch.as_tensor(_Buf(), device=device)
+
+
 def prefix_length(preassembled):
     """`preassembled` of config/furniture.py:158 -> how many recipe steps it names.  The accelerated path starts an episode after the first k
     steps of the recipe, which is what set_subtask produces (furniture.py:204-207) and what the dense reward assumes
@@ -250,6 +261,11 @@ class BatchedFurnitureEnv:
         self._done = torch.empty(num_envs, dtype=torch.uint8, device=self.device)
         self._info = torch.empty((num_envs, INFO_DIM), dtype=torch.int32, device=self.device)
         self._act = torch.empty((num_envs, self.act_dim), dtype=torch.float32, device=self.device)
+        # the engine's terminal buffers, which the step kernel writes for every env whose step ends an episode (the layout is fixed by now)
+        tob, tq, tv = e.terminal_dev_ptrs()
+        self._term_obs = device_view(tob, (num_envs, self.obs_dim), self.device)
+        self._term_qpos = device_view(tq, (num_envs, self.model.nq), self.device)
+        self._term_qvel = device_view(tv, (num_envs, self.model.nv), self.device)
 
     def set_init_qpos(self, states):
         """FurnitureEnv.set_init_qpos (furniture.py:315-316), per env: one get_env_state dict or None for all envs, or a list of num_envs of
@@ -354,6 +370,18 @@ class BatchedFurnitureEnv:
         obs, rew, done, info = self.engine.env_step_host(actions_np)
         return self._obs_dict(obs), rew, done.astype(bool), info
 
+    def terminal_observation(self):
+        """the observation FurnitureEnv.step returns with done (furniture.py:364-385), which step() cannot return because the env is already
+        reset into its next episode: an obs dict with step()'s keys and columns, views of the device buffer the step kernel writes before the
+        auto-reset (the two-arm IK / controller robot_ob is gathered, as in step()).  Row i is valid where the last step's done[i] is 1; after an
+        unstable step it is the observation of the reset inside _do_simulation's except branch (furniture.py:2889-2897), as the reference's."""
+        return self._obs_dict(self._term_obs)
+
+    def terminal_state(self):
+        """{"qpos" (N, nq), "qvel" (N, nv)}: what get_env_state would have returned at the end of each episode that the last step finished,
+        views of the device buffers, valid where that step's done is 1"""
+        return {"qpos": self._term_qpos, "qvel": self._term_qvel}
+
     def infos(self):
         info = self._info.cpu().numpy()
         return tuple({k: int(row[j]) for j, k in enumerate(INFO_KEYS)} for row in info)
@@ -433,6 +461,10 @@ class MixedFurnitureEnv:
         self._info = torch.empty((off, INFO_DIM), dtype=torch.int32, device=self.device)
         self._act = torch.empty((off, self.act_dim), dtype=torch.float32, device=self.device)
         self._streams = [torch.cuda.Stream(device=self.device) for _ in self.buckets]
+        self._term_obs = torch.zeros_like(self._obs)  # terminal_observation's rows, laid out like _obs
+        self._term_views, o = OrderedDict(), 0
+        for k, w in widths.items():
+            self._term_views[k], o = self._term_obs[:, o : o + w], o + w
 
     def set_sim_options(self, control_freq=None, no_collision=None, envs=None):
         """BatchedFurnitureEnv.set_sim_options with `envs` as global indices of this batch (default: all); each value is a scalar or one
@@ -511,6 +543,19 @@ class MixedFurnitureEnv:
 
         self._fan_out(one)
         return self._obs_dict(self._obs), self._rew, self._done, self._info
+
+    def terminal_observation(self):
+        """BatchedFurnitureEnv.terminal_observation of every bucket, gathered in global env order with step()'s layout (object_ob zero-padded to
+        the batch's width, or 14 wide without object_ob_all); row i is valid where the last step's done[i] is 1"""
+        for b, off in zip(self.buckets, self.offsets):
+            for k, v in b.terminal_observation().items():
+                self._term_views[k][off : off + b.num_envs, : v.shape[1]].copy_(v)
+        return self._obs_dict(self._term_obs)
+
+    def terminal_state(self):
+        """BatchedFurnitureEnv.terminal_state of every bucket, in bucket order (bucket i holds the envs from offsets[i] on): the models' nq and nv
+        differ, so the states are not stacked"""
+        return [b.terminal_state() for b in self.buckets]
 
     def close(self):
         for b in self.buckets:

@@ -6,11 +6,17 @@
   ob, reward, done, info = env.step(action)         # action: (dof,) array or {"default": array}
 
 It is the batched engine with one env (the batch entry point `furniture_b200.env.make_vec_env` is the one to use for
-throughput).  Differences from the reference, all consequences of the step kernel resetting a finished env on the
-device like a `SubprocVecEnv` worker does (subproc_vec_env.py:16-20):
-  * the observation returned together with `done=True` is the first observation of the next episode, not the terminal one;
-  * the `reset()` the caller issues after `done` returns that same observation and does not reset a second time, so the
-    env consumes exactly one reset's worth of numpy random draws per episode, like the reference (furniture.py:72).
+throughput).  The step kernel resets a finished env on the device in the same launch, like a `SubprocVecEnv` worker
+does (subproc_vec_env.py:16-20).  The `reset()` the caller issues after `done` returns the first observation of the
+episode the device has already started and does not reset a second time, so the env consumes exactly one reset's worth
+of numpy random draws per episode, like the reference (furniture.py:72).  What `step` returns with `done=True` depends
+on the keyword `terminal_observation`:
+  * False (the default): the first observation of the next episode, not the terminal one, and `get_env_state()` gives
+    the state of that next episode -- the difference from the reference's `FurnitureEnv.step`;
+  * True: the terminal observation, as the reference's `FurnitureEnv.step` returns it (furniture.py:364-385), and
+    `get_env_state()` gives the terminal state until the caller's `reset()`.  The step kernel writes both before its
+    auto-reset; after an unstable step they are those of the reset inside `_do_simulation`'s except branch
+    (furniture.py:2889-2897), as in the reference.
 `info` carries the reference's episode keys at the end of an episode (`_after_step`, furniture.py:451-480).
 """
 from __future__ import annotations
@@ -24,9 +30,11 @@ import numpy as np
 class FurnitureGymB200:
     metadata = {"render.modes": []}
 
-    def __init__(self, name="FurnitureSawyerEnv", furniture_name=None, device=0, lib_path=None, id=None, **config):
+    def __init__(self, name="FurnitureSawyerEnv", furniture_name=None, device=0, lib_path=None, id=None, terminal_observation=False, **config):
         """`id`, `name` and the remaining keywords are what gym passes from the registration (env/__init__.py:19-114: id, name,
-        furniture_name / furniture_id, background, port ...); options of the renderer are ignored, see env.split_config"""
+        furniture_name / furniture_id, background, port ...); options of the renderer are ignored, see env.split_config.
+        `terminal_observation`: step returns the terminal observation with done=True, as the reference's FurnitureEnv.step does (see the
+        module's docstring)"""
         from .env import ENV_IDS, build_engine, env_options
 
         ids = dict(ENV_IDS, Sawyer=ENV_IDS["FurnitureSawyerEnv"], Baxter=ENV_IDS["FurnitureBaxterEnv"])  # and the bare agent names
@@ -44,6 +52,8 @@ class FurnitureGymB200:
         self.object_ob_dim, self.subtask_ob_dim, self.robot_ob_dim, self.phase_ob_dim = (widths[k] for k in ("object_ob", "subtask_ob", "robot_ob", "phase_ob"))
         self._max_episode_steps = self.cfg.max_episode_steps
         self._pending_ob = None  # observation of an episode the device has already started
+        self._terminal = bool(terminal_observation)
+        self._terminal_state = None  # with terminal_observation: the state the finished episode ended in, until reset()
         self._episode_reward = 0.0
         self._episode_time = time.time()
 
@@ -71,6 +81,7 @@ class FurnitureGymB200:
         return OrderedDict((k, obs_row[c].astype(np.float64)) for k, c in self._cols.items())
 
     def reset(self):
+        self._terminal_state = None
         if self._pending_ob is not None:
             ob, self._pending_ob = self._pending_ob, None
         else:
@@ -86,6 +97,7 @@ class FurnitureGymB200:
         a = np.asarray(action, dtype=np.float32).reshape(1, self.dof)
         if self._pending_ob is not None:  # stepping on after `done` without reset(): the device is already in the next episode
             self._pending_ob, self._episode_reward, self._episode_time = None, 0.0, time.time()
+            self._terminal_state = None
         obs, rew, done, info = self.engine.env_step_host(a)
         reward, done = float(rew[0]), bool(done[0])
         self._episode_reward += reward
@@ -105,6 +117,10 @@ class FurnitureGymB200:
             out["episode_unstable"] = -float(self.cfg.unstable_penalty_coef) if unstable else 0
             out["episode_num_connected"] = int(info[0][0])
             self._pending_ob = ob
+            if self._terminal:  # the row and the state the step kernel kept before its auto-reset
+                ob = self._ob(self.engine.terminal_obs()[0])
+                q, v = self.engine.terminal_state()
+                self._terminal_state = {"qpos": q[0].astype(np.float64), "qvel": v[0].astype(np.float64)}
         return ob, reward, done, out
 
     # ---- pass-throughs of FurnitureGym (furniture_gym.py:35-50)
@@ -137,10 +153,13 @@ class FurnitureGymB200:
         self._pending_ob = None
 
     def get_env_state(self):
+        if self._terminal_state is not None:
+            return {k: v.copy() for k, v in self._terminal_state.items()}
         q, v = self.engine.get_state()
         return {"qpos": q[0].astype(np.float64), "qvel": v[0].astype(np.float64)}
 
     def set_env_state(self, state):
+        self._terminal_state = None
         self.engine.set_state(np.asarray(state["qpos"])[None], np.asarray(state["qvel"])[None])
         self.engine.set("ctrl", np.zeros((1, self.model.nu), np.float32))
         self.engine.forward()

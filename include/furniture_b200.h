@@ -20,6 +20,8 @@
  *   fe_dense_eval    <- the same reward machine on explicit poses (test hook)          furniture_sawyer_dense.py:225-586
  *   fe_set_obs_layout <- the observation flags robot_ob / object_ob / object_ob_all / subtask_ob, with _get_next_subtask
  *                       tracked per env inside the kernels    furniture.py:103-107, :215-252, :1344-1387, :2723-2759
+ *   fe_terminal_obs_dev / fe_terminal_qpos_dev / fe_terminal_qvel_dev <- the terminal `ob` of FurnitureEnv.step and the state
+ *                       get_env_state gives at that point     furniture.py:364-385, :1781-1792
  *
  * Conventions: every function returns 0 on success or a negative code and records a message retrievable with
  * fe_last_error(); a handle is bound to one CUDA device, is not thread-safe, and all work is issued on the stream
@@ -223,6 +225,18 @@ int fe_set_obs_layout(fe_handle* h, int robot_ob, int object_ob, int object_ob_a
 int fe_dense_info_dim(void);
 /* device pointer of the internal obs buffer after the last step/reset: (n_envs, obs_dim) float32 */
 const float* fe_obs_dev(const fe_handle* h);
+/* What an episode left when it ended: the reference's FurnitureEnv.step returns the terminal observation with done (furniture.py:364-385),
+ * while the env steps here reset a finished env in the same launch and return the next episode's first observation.  Every env step
+ * (fe_env_step, fe_env_step_packed, fe_env_step_host, under every control type) writes, for each env whose step returns done = 1, the
+ * observation row that step would have returned without the reset into terminal_obs (n_envs, obs_dim) float32, and its qpos / qvel into
+ * terminal_qpos (n_envs, nq) / terminal_qvel (n_envs, nv) float32, before the auto-reset.  After an unstable step these hold the world of the
+ * reset inside _do_simulation's except branch, which is what the reference's step returns (furniture.py:2889-2897).  A row is valid where
+ * the last step's done is 1; the rows of the other envs, and every row after fe_env_reset, are left as they are.  The same arrays are the
+ * read-only fields "terminal_obs", "terminal_qpos" and "terminal_qvel"; fe_set_obs_layout reallocates terminal_obs with obs (the pointer
+ * moves).  A handle created without a scene blob has neither the fields nor the buffers: the accessors return NULL. */
+const float* fe_terminal_obs_dev(const fe_handle* h);
+const float* fe_terminal_qpos_dev(const fe_handle* h);
+const float* fe_terminal_qvel_dev(const fe_handle* h);
 
 /* ---- test hook: the device _is_aligned on explicit site poses (float64), n independent cases */
 int fe_is_aligned(fe_handle* h, int n, const double* p1, const double* m1, const double* p2, const double* m2, const double* angles /* (n,4) */,
