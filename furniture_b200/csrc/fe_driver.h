@@ -24,6 +24,9 @@ struct FeState {
 struct FeDebug {
   float *Mr, *fs, *as, *linert, *x, *fc, *c_dist, *c_pos, *c_frame, *c_aref, *c_D, *c_f, *lmat, *S;
   int *c_geom, *c_state;
+  float *c_mu, *c_fric;                 // [N][maxcon] regularised and plain friction coefficient of each contact
+  float *w_aref, *w_D, *w_f;            // [N][6 neq] weld rows (3 translational, 3 rotational); rows of inactive welds are stale
+  float *l_sign, *l_aref, *l_D, *l_f;   // [N][nr] joint-limit rows: side (+1 lower, -1 upper, 0 none), aref, D, force
 };
 
 FE_FN void fe_load(FeWarp* w, const FeState& s, int env) {
@@ -56,6 +59,8 @@ FE_FN void fe_dump(FeWarp* w, const FeDebug& d, int env) {
   LANES_BEGIN
     DP(Mr, m->nr * m->nr) DP(fs, m->nv) DP(as, m->nv) DP(linert, 10 * m->nlink) DP(x, m->nv) DP(fc, m->nv) DP(lmat, 9 * m->nlink) DP(S, 6 * m->nr)
     DP(c_dist, mc) DP(c_pos, 3 * mc) DP(c_aref, 3 * mc) DP(c_D, 2 * mc) DP(c_f, 3 * mc) DP(c_geom, mc) DP(c_state, mc)
+    DP(c_mu, mc) DP(c_fric, mc) DP(w_aref, 6 * m->neq) DP(w_D, 6 * m->neq) DP(w_f, 6 * m->neq)
+    DP(l_sign, m->nr) DP(l_aref, m->nr) DP(l_D, m->nr) DP(l_f, m->nr)
     if (d.c_frame) for (int c = lane; c < mc; c += 32) { float F[9]; fe_frame_load(w, c, F); for (int k = 0; k < 9; ++k) d.c_frame[(size_t)env * 9 * mc + 9 * c + k] = F[k]; }
   LANES_END
 #undef DP

@@ -38,7 +38,7 @@ NEAR = 1e-5  # fp32 and fp64 may disagree on whether a contact this close to its
 # ---------------------------------------------------------------- the dispatch rule of fe_solve, restated
 def classify(m, em, contacts, eq_active):
     """fe_solve's decision for one constraint set.  Contact kind as in fe_assemble: 0 a free part against the static world,
-    1 robot only, 2 robot against a part, 3 part against part."""
+    1 robot only, 2 robot against a part, 3 part against part; `kinds` per contact, `cpl` per part (in the coupled component)."""
     nrl, npart, nr = em.nrlink, em.npart, em.nrlink
     link = lambda g: em.weld_link(int(m.geom_bodyid[g]))
     kinds, owner = [], []
@@ -69,7 +69,7 @@ def classify(m, em, contacts, eq_active):
     cpl = [touch[p] or welded[p] or nstat[p] > 8 for p in range(npart)]
     nA = (nr if robot_in else 0) + 6 * sum(cpl)
     ncc = sum(1 for k, p in zip(kinds, owner) if k != 0 or cpl[p])
-    info = dict(nA=nA, ncc=ncc, ncpl=sum(cpl), nstat=nstat, robot_in=robot_in, weld=any(welded), ncon=len(contacts))
+    info = dict(nA=nA, ncc=ncc, ncpl=sum(cpl), nstat=nstat, robot_in=robot_in, weld=any(welded), ncon=len(contacts), kinds=kinds, cpl=cpl)
     if not any(cpl) and not robot_in:
         units, passes, p0 = [], 0, 0
         while p0 < npart:  # fe_solve_parts_grouped's packing: 8 units of 4 lanes per pass, a wide part on an aligned pair
