@@ -32,13 +32,18 @@ STAT_NEWTON_SETUP, STAT_NEWTON_START, STAT_NEWTON_GRAD, STAT_NEWTON_HESSIAN, STA
 i32, f32, f64 = C.c_int32, C.c_float, C.c_double
 # the observation flags of config/furniture.py:228-258 and their defaults; other values go to fe_set_obs_layout
 OBS_DEFAULTS = dict(robot_ob=True, object_ob=True, object_ob_all=True, subtask_ob=False)
-# the task options of config/furniture.py (:95-100, :163-168, :177-194, :203-226, :291-295) -> (per-env field, column); see set_task_options
-TASK_OPTIONS = dict(
-    alignment_pos_dist=("alignment", 0), alignment_rot_dist_up=("alignment", 1), alignment_rot_dist_forward=("alignment", 2),
-    alignment_project_dist=("alignment", 3), auto_align=("auto_align", 0), furn_xyz_rand=("placement_rand", 0),
-    furn_rot_rand=("placement_rand", 1), agent_xyz_rand=("placement_rand", 2), success_reward=("reward_coef", 0),
-    touch_reward=("reward_coef", 1), pick_reward=("reward_coef", 2), ctrl_penalty_coef=("reward_coef", 3),
-    unstable_penalty_coef=("reward_coef", 4), max_episode_steps=("max_episode_steps", 0))
+# the per-env options of config/furniture.py by their key names -> (per-env field, column, converter from the caller's value to the field's,
+# or None); Engine._set_options writes them.  The reset options (:116-127, :169-174, :307-312), the sim options (:71-73, :304-306) and the
+# task options (:95-100, :163-168, :177-194, :203-226, :291-295).
+OPTIONS = dict(
+    fix_init=("fix_init", 0, None), fix_init_parts=("fix_init_parts", 0, lambda eng, parts: eng.part_mask(parts)),
+    reset_robot_after_attach=("reset_robot_after_attach", 0, None), assembled=("assembled", 0, None),
+    control_freq=("substeps", 0, lambda eng, freq: eng.substeps(freq)), no_collision=("no_collision", 0, lambda eng, v: np.asarray(v, dtype=bool)),
+    alignment_pos_dist=("alignment", 0, None), alignment_rot_dist_up=("alignment", 1, None), alignment_rot_dist_forward=("alignment", 2, None),
+    alignment_project_dist=("alignment", 3, None), auto_align=("auto_align", 0, None), furn_xyz_rand=("placement_rand", 0, None),
+    furn_rot_rand=("placement_rand", 1, None), agent_xyz_rand=("placement_rand", 2, None), success_reward=("reward_coef", 0, None),
+    touch_reward=("reward_coef", 1, None), pick_reward=("reward_coef", 2, None), ctrl_penalty_coef=("reward_coef", 3, None),
+    unstable_penalty_coef=("reward_coef", 4, None), max_episode_steps=("max_episode_steps", 0, None))
 
 
 class FeConfig(C.Structure):
@@ -49,6 +54,10 @@ class FeConfig(C.Structure):
         ("ctrl_penalty_coef", f32), ("unstable_penalty_coef", f32), ("success_reward", f32), ("touch_reward", f32), ("pick_reward", f32),
         ("furn_xyz_rand", f32), ("furn_rot_rand", f32), ("agent_xyz_rand", f32), ("furn_size_rand", f32), ("seed", C.c_uint64),
     ]
+
+
+# the task options (set_task_options): the per-env options that start from the FeConfig member of the same name
+TASK_OPTIONS = tuple(k for k in OPTIONS if hasattr(FeConfig, k))
 
 
 class FeScene(C.Structure):
@@ -255,6 +264,8 @@ class Engine:
         self.L = L
         L.fe_last_error.restype = C.c_char_p
         L.fe_last_error.argtypes = [C.c_void_p]
+        L.fe_field_dtype.restype = C.c_char_p
+        L.fe_field_dtype.argtypes = [C.c_void_p, C.c_char_p]
         for f in ("fe_model_sizeof", "fe_scene_sizeof", "fe_config_sizeof"):
             getattr(L, f).restype = C.c_size_t
         for f in ("fe_obs_dev", "fe_terminal_obs_dev", "fe_terminal_qpos_dev", "fe_terminal_qvel_dev"):
@@ -333,17 +344,11 @@ class Engine:
         if assembled is not None and self.model.meta.get("agent") == "Cursor":
             raise ValueError("assembled is built for the robot envs; the Cursor env's reset is host logic (cursor_env.FurnitureCursorEnvB200)")
         partial = self._xml_listed and self._xml_listed != set(self.em.part_names)
-        if partial and (fix_init or set(self._part_names(fix_init_parts)) - self._xml_listed):  # init_pos[body]: the reference's KeyError
+        if partial and (np.any(fix_init) or set(self._part_names(fix_init_parts)) - self._xml_listed):  # init_pos[body]: the reference's KeyError
             raise ValueError("the XML of %s lists init poses for some parts only: fix_init, and fix_init_parts beyond %s, are undefined there"
                              % (self.model.meta.get("furniture"), sorted(self._xml_listed)))
-        idx = np.arange(self.N) if envs is None else np.asarray(envs, dtype=np.int64).ravel()
-        for name, v in (("fix_init", fix_init), ("fix_init_parts", None if fix_init_parts is None else self.part_mask(fix_init_parts)),
-                        ("reset_robot_after_attach", reset_robot_after_attach), ("assembled", assembled)):
-            if v is None:
-                continue
-            cur = self.get(name)
-            cur[idx, 0] = int(v)
-            self.set(name, cur)
+        self._set_options(envs, dict(fix_init=fix_init, fix_init_parts=fix_init_parts, reset_robot_after_attach=reset_robot_after_attach,
+                                     assembled=assembled))
 
     def substeps(self, control_freq):
         """substep_count at this model's timestep"""
@@ -357,14 +362,7 @@ class Engine:
         if self.model.meta.get("agent") == "Cursor":
             raise ValueError("the Cursor env takes its own control_freq (cursor_env.FurnitureCursorEnvB200); control_freq and no_collision "
                              "are options of the robot envs")
-        idx = np.arange(self.N) if envs is None else np.asarray(envs, dtype=np.int64).ravel()
-        for name, v in (("substeps", None if control_freq is None else self.substeps(control_freq)),
-                        ("no_collision", None if no_collision is None else np.asarray(no_collision, dtype=bool).astype(np.int32))):
-            if v is None:
-                continue
-            cur = self.get(name)
-            cur[idx, 0] = v
-            self.set(name, cur)
+        self._set_options(envs, dict(control_freq=control_freq, no_collision=no_collision))
 
     def set_task_options(self, envs=None, **values):
         """the task options of config/furniture.py for the envs in `envs` (default: all), each a scalar or one value per env of `envs`, by the
@@ -378,22 +376,27 @@ class Engine:
         unknown = sorted(set(values) - set(TASK_OPTIONS))
         if unknown:
             raise ValueError("unknown task options %s (known: %s)" % (unknown, sorted(TASK_OPTIONS)))
+        self._set_options(envs, values)
+
+    def _set_options(self, envs, values):
+        """writes `values` (OPTIONS keys -> a scalar or one value per env of `envs`; None leaves an option as it is) for the envs in `envs`
+        (default: all).  Every value is checked and converted before any field is written, and each field touched is written once."""
         idx = np.arange(self.N) if envs is None else np.asarray(envs, dtype=np.int64).ravel()
         if idx.size and (idx.min() < 0 or idx.max() >= self.N):
             raise IndexError("envs must lie in [0, %d), got %s" % (self.N, idx.tolist()))
-        fields = {}
+        columns = {}
         for key, v in values.items():
             if v is None:
                 continue
-            name, col = TASK_OPTIONS[key]
-            if name not in fields:
-                fields[name] = self.get(name)
-            cur = fields[name]
-            v = np.asarray(v)
+            name, col, convert = OPTIONS[key]
+            v = np.asarray(v if convert is None else convert(self, v))
             if v.ndim > 1 or (v.ndim == 1 and v.shape != idx.shape):
                 raise ValueError("%s takes a scalar or one value per env of `envs` (%d), got shape %s" % (key, idx.size, v.shape))
-            cur[idx, col] = v.astype(cur.dtype)
-        for name, cur in fields.items():
+            columns.setdefault(name, []).append((col, v))
+        for name, cols in columns.items():
+            cur = self.get(name)
+            for col, v in cols:
+                cur[idx, col] = v.astype(cur.dtype)
             self.set(name, cur)
 
     def close(self):
@@ -417,28 +420,19 @@ class Engine:
         self._chk(self.L.fe_field_dim(self.h, name.encode(), C.byref(d), C.byref(e)))
         return d.value, e.value
 
-    _INT = {"order", "geom_contype", "geom_conaffinity", "eq_active", "touch", "flags", "ncon", "niter", "stats", "con_geom", "con_state", "group", "site_connected",
-            "num_connected", "prev_num_connected", "touched", "picked", "episode_length", "done", "mt_pos", "preassembled", "num_connects",
-            "init_state", "init_pick", "init_mt_pos", "subtask_part", "fix_init", "fix_init_parts", "fix_have", "reset_robot_after_attach",
-            "substeps", "no_collision", "assembled", "auto_align", "max_episode_steps"}
-    _U32 = {"mt_state", "init_mt_state"}
-    _F64 = {"fix_pose", "alignment"}
-
-    def _dtype(self, name, eb):
-        if eb == 8:
-            return np.float64 if name in self._F64 else np.uint64
-        return np.uint8 if eb == 1 else (np.uint32 if name in self._U32 else (np.int32 if name in self._INT else np.float32))
+    def _dtype(self, name):
+        """the field's element type as the library registers it (after field_info, which refuses an unknown name)"""
+        return np.dtype(self.L.fe_field_dtype(self.h, name.encode()).decode())
 
     def get(self, name):
-        dim, eb = self.field_info(name)
-        out = np.empty((self.N, dim), dtype=self._dtype(name, eb))
+        dim, _ = self.field_info(name)
+        out = np.empty((self.N, dim), dtype=self._dtype(name))
         self._chk(self.L.fe_get_field(self.h, name.encode(), out.ctypes.data_as(C.c_void_p), C.c_size_t(out.nbytes)))
         return out
 
     def set(self, name, value):
-        dim, eb = self.field_info(name)
-        dt = self._dtype(name, eb)
-        v = np.ascontiguousarray(np.broadcast_to(np.asarray(value, dtype=dt), (self.N, dim)))
+        dim, _ = self.field_info(name)
+        v = np.ascontiguousarray(np.broadcast_to(np.asarray(value, dtype=self._dtype(name)), (self.N, dim)))
         self._chk(self.L.fe_set_field(self.h, name.encode(), v.ctypes.data_as(C.c_void_p), C.c_size_t(v.nbytes)))
 
     def get_state(self):

@@ -81,8 +81,7 @@ def split_config(config):
     if name is None and cfg.get("furniture_id") is not None:
         name = FURNITURE_NAMES[int(cfg["furniture_id"])]
     fields = {f[0] for f in FeConfig._fields_} - {"struct_bytes"}
-    renamed = {"furn_xyz_rand": "furn_xyz_rand", "furn_rot_rand": "furn_rot_rand", "agent_xyz_rand": "agent_xyz_rand", "alignment_pos_dist": "alignment_pos_dist"}
-    over = {renamed.get(k, k): v for k, v in cfg.items() if renamed.get(k, k) in fields and v is not None}
+    over = {k: v for k, v in cfg.items() if k in fields and v is not None}
     ignored = sorted(k for k in cfg if k not in over and k not in ("furniture_name", "furniture_id", "control_type", "preassembled", "num_connects",
                                                                    "load_init_states", "load_demo") + tuple(OBS_DEFAULTS) + tuple(RESET_DEFAULTS)
                      + tuple(SIM_DEFAULTS))
@@ -189,11 +188,6 @@ def build_engine(agent, furniture_name, num_envs, device=0, lib_path=None, dense
     The other keywords override FeConfig fields (default_config).  The engine records `control_type` and `resize_factor`."""
     if control_freq is not None and "nsub" in cfg_overrides:
         raise ValueError("control_freq and nsub both set the mj_steps of an env step: give one of them")
-    if agent == "Cursor" and assembled:
-        raise ValueError("assembled is built for the robot envs; the Cursor env's reset is host logic (cursor_env.FurnitureCursorEnvB200)")
-    if agent == "Cursor" and (control_freq is not None or np.any(no_collision)):
-        raise ValueError("the Cursor env takes its own control_freq (cursor_env.FurnitureCursorEnvB200); control_freq and no_collision "
-                         "are options of the robot envs")
     per_env = {k: cfg_overrides.pop(k) for k in list(cfg_overrides) if k in TASK_OPTIONS and np.ndim(cfg_overrides[k]) > 0}
     cfg = default_config(**cfg_overrides)
     # furn_size_rand (config/furniture.py:196-201): the reference draws one size factor per env process while loading the model.
@@ -469,17 +463,16 @@ class MixedFurnitureEnv:
     def set_sim_options(self, control_freq=None, no_collision=None, envs=None):
         """BatchedFurnitureEnv.set_sim_options with `envs` as global indices of this batch (default: all); each value is a scalar or one
         per env of `envs`"""
-        idx = np.arange(self.real_envs) if envs is None else np.asarray(envs, dtype=np.int64).ravel()
-        per = lambda v: None if v is None else np.broadcast_to(np.asarray(v), idx.shape)
-        cf, nc = per(control_freq), per(no_collision)
-        for b, off in zip(self.buckets, self.offsets):
-            sel = (idx >= off) & (idx < off + b.num_envs)
-            if sel.any():
-                b.set_sim_options(None if cf is None else cf[sel], None if nc is None else nc[sel], idx[sel] - off)
+        self._per_bucket(envs, dict(control_freq=control_freq, no_collision=no_collision), lambda b, idx, v: b.set_sim_options(envs=idx, **v))
 
     def set_task_options(self, envs=None, **values):
         """BatchedFurnitureEnv.set_task_options with `envs` as global indices of this batch (default: all); each value is a scalar or one
         per env of `envs`"""
+        self._per_bucket(envs, values, lambda b, idx, v: b.set_task_options(idx, **v))
+
+    def _per_bucket(self, envs, values, set_options):
+        """set_options(bucket, its envs, their values) for every bucket that holds some of `envs` (global indices, default: all), each of
+        `values` a scalar or one per env of `envs` (None: left out)"""
         idx = np.arange(self.real_envs) if envs is None else np.asarray(envs, dtype=np.int64).ravel()
         if idx.size and (idx.min() < 0 or idx.max() >= self.real_envs):
             raise IndexError("envs must lie in [0, %d), got %s" % (self.real_envs, idx.tolist()))
@@ -487,7 +480,7 @@ class MixedFurnitureEnv:
         for b, off in zip(self.buckets, self.offsets):
             sel = (idx >= off) & (idx < off + b.num_envs)
             if sel.any():
-                b.set_task_options(idx[sel] - off, **{k: v[sel] for k, v in per.items()})
+                set_options(b, idx[sel] - off, {k: v[sel] for k, v in per.items()})
 
     def _obs_dict(self, obs):
         d, o = OrderedDict(), 0

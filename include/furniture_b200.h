@@ -136,6 +136,9 @@ int fe_sim_step(fe_handle* h, int nsub, void* stream);
 int fe_get_field(fe_handle* h, const char* name, void* dst_host, size_t bytes);
 int fe_set_field(fe_handle* h, const char* name, const void* src_host, size_t bytes);
 int fe_field_dim(fe_handle* h, const char* name, int* dim, int* elem_bytes);
+/* the numpy typestr of one element of field `name`: "<i4" (int32), "<u4" (uint32), "<f4" (float32), "<f8" (float64) or "|u1" (bytes, the
+   struct-valued fields ik_state, ctl_state and dense_state); NULL for an unknown name, with fe_last_error set */
+const char* fe_field_dtype(fe_handle* h, const char* name);
 int fe_get_state(fe_handle* h, float* qpos_host, float* qvel_host);
 int fe_set_state(fe_handle* h, const float* qpos_host, const float* qvel_host);
 /* Recorded starts, FurnitureEnv._init_qpos (furniture.py:121-130, :315-316, :1433-1434, :1505-1518, :1617): a bank of n_states
