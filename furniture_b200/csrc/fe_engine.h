@@ -2234,7 +2234,7 @@ FE_FN void fe_substep(FeWarp* w) {
 // same step with block barriers between the phases: the warps (= envs) of a block then fetch the same instructions at the
 // same time, which is what keeps the instruction cache effective for this large, mostly straight-line code.  Every live warp
 // of the block must reach the same sequence of barriers: the step loops of the env steps, whose length is the env's own
-// substep count, keep it with fe_block_any and fe_substep_idle (below); fe_run_env runs one count for the whole launch.
+// substep count, keep it with fe_substeps_mixed (below); fe_run_env runs one count for the whole launch.
 FE_FN void fe_substep_lockstep(FeWarp* w) {
   FE_TICK_START
   FE_BLOCK_SYNC; FE_TICK(w->u() + FE_U_STAT, FE_STAT_WAIT, FE_STAT_WAIT_KIN) fe_kin_smooth(w); FE_TICK(w->u() + FE_U_STAT, FE_STAT_KIN)
@@ -2247,8 +2247,7 @@ FE_FN void fe_substep_lockstep(FeWarp* w) {
   FE_TICK(w->u() + FE_U_STAT, FE_STAT_SOLVE)
   FE_BLOCK_SYNC; FE_TICK(w->u() + FE_U_STAT, FE_STAT_WAIT, FE_STAT_WAIT_INTEGRATE) fe_integrate(w); FE_TICK(w->u() + FE_U_STAT, FE_STAT_INTEGRATE)
 }
-// A step loop whose trip count differs between the warps of a block (each env's substeps) runs as
-//   for (int i = 0; fe_block_any(i < n); ++i) { if (i < n) fe_substep_lockstep(w); else fe_substep_idle(); }
+// A step loop whose trip count differs between the warps of a block (each env's substeps) is fe_substeps_mixed, below.
 // Every live warp runs the block's largest count of iterations: one whose own steps are done passes the five barriers of a step
 // without the step.  The loop test is a barrier itself (bar.red.or on sm_90a), reached by every live thread once per iteration, and
 // its result is the same on every thread, so the block's threads all leave the loop after the same iteration and every barrier
@@ -2262,3 +2261,9 @@ FE_HD bool fe_block_any(bool p) {
 #endif
 }
 FE_HD void fe_substep_idle() { FE_BLOCK_SYNC; FE_BLOCK_SYNC; FE_BLOCK_SYNC; FE_BLOCK_SYNC; FE_BLOCK_SYNC; }
+// the env's `n` mj_steps in a block whose warps may run different counts
+FE_HD void fe_substeps_mixed(FeWarp* w, int n) {
+  for (int i = 0; fe_block_any(i < n); ++i) {
+    if (i < n) fe_substep_lockstep(w); else fe_substep_idle();
+  }
+}

@@ -354,13 +354,16 @@ FE_HDN void fe_site_pose_d(const FeWarp* w, int site, double* pos, double* mat, 
   }
 }
 
+// _finger_contact: both fingers of arm `arm` touch the part whose touch bits are `t` (bits 0 / 1: arm 0's fingers, 3 / 4: arm 1's)
+FE_HD bool fe_both_fingers(int t, int arm) { const int both = arm == 0 ? 3 : 24; return (t & both) == both; }
+
 // the dense reward's view of the env: poses of the last forward pass, as _get_obs and the connect scan see them
 struct FeSliceWorld {
   const FeWarp* w;
   FE_MEMBER void site_pos(int s, double* p) const { fe_site_pose_d(w, s, p, nullptr, nullptr); }
   FE_MEMBER void site_pose(int s, double* p, double* m) const { fe_site_pose_d(w, s, p, m, nullptr); }
   FE_MEMBER void part_pos(int q, double* p) const { const float* lp = w->lpos() + 3 * (w->m->nrlink + q); p[0] = (double)lp[0]; p[1] = (double)lp[1]; p[2] = (double)lp[2]; }
-  FE_MEMBER bool touch_both(int q) const { return (w->touch()[q] & 3) == 3; } // _finger_contact(leg): both fingers of the (only) arm
+  FE_MEMBER bool touch_both(int q) const { return fe_both_fingers(w->touch()[q], 0); } // _finger_contact(leg): the (only) arm
 };
 
 // _stop_object(obj, gravity=gc): xfrc_applied -> gravity-compensation factor, qvel = 0 (furniture.py:2778-2800)
@@ -369,8 +372,10 @@ FE_HD void fe_stop_part(FeWarp* w, int p, float gc) {
   w->gravcomp()[p] = gc;
   for (int k = 0; k < 6; ++k) w->qvel()[da + k] = 0.f;
 }
-// _move_objects_translation_quat(obj, translation, target_quat, gravity): rigidly move obj's whole group (furniture.py:1163-1176)
-FE_HDN void fe_move_group(FeEnv* e, int obj, const double* translation, const double* target_quat, float gc) {
+// _move_objects_translation_quat(obj, translation, target_quat, gravity=0): rigidly move obj's whole group and stop every part of it
+// (furniture.py:1163-1176).  Without `stop` it is the move of _move_rotate_object, which keeps the parts' velocities and gravity compensation.
+// A null target_quat is obj's own quaternion.
+FE_HDN void fe_move_group(FeEnv* e, int obj, const double* translation, const double* target_quat, bool stop) {
   FeWarp* w = e->w;
   const fe_model* m = w->m;
   const int qb = m->link_qadr[m->nrlink + obj];
@@ -382,10 +387,10 @@ FE_HDN void fe_move_group(FeEnv* e, int obj, const double* translation, const do
     const int qa = m->link_qadr[m->nrlink + i];
     double q[7], np_[3], nq[4];
     for (int k = 0; k < 7; ++k) q[k] = (double)w->qpos()[qa + k];
-    d_transform_to_target(base, q, target_quat, np_, nq);
+    d_transform_to_target(base, q, target_quat ? target_quat : base + 3, np_, nq);
     for (int k = 0; k < 3; ++k) w->qpos()[qa + k] = (float)(np_[k] + translation[k]);
     for (int k = 0; k < 4; ++k) w->qpos()[qa + 3 + k] = (float)nq[k];
-    fe_stop_part(w, i, gc);
+    if (stop) fe_stop_part(w, i, 0.f);
   }
 }
 // min z over every site of every part in obj's group, starting from 0 (furniture.py:749-769)
@@ -480,15 +485,12 @@ FE_FN void fe_connect(FeEnv* e, int align) {
         for (int k = 0; k < 3; ++k) base[k] = sp[k];
         for (int k = 0; k < 4; ++k) base[3 + k] = sq[k];
         const int qa = m->link_qadr[m->nrlink + body2];
-        double bq[7], np_[3], nq[4], nsp[3], nsq[4], nb[7];
+        double bq[7], np_[3], nq[4], nsp[3], nsq[4];
         for (int k = 0; k < 7; ++k) bq[k] = (double)w->qpos()[qa + k];
         d_transform_to_target(base, bq, target + 3, np_, nq);
-        for (int k = 0; k < 3; ++k) nb[k] = bq[k];
-        for (int k = 0; k < 4; ++k) nb[3 + k] = bq[3 + k];
         d_transform_to_target(bq, base, nq, nsp, nsq);
         double tr[3] = {target[0] - nsp[0], target[1] - nsp[1], target[2] - nsp[2]};
-        fe_move_group(e, body2, tr, nq, 0.f);
-        (void)nb;
+        fe_move_group(e, body2, tr, nq, true);
       }
     }
   LANES_END
@@ -507,23 +509,8 @@ FE_FN void fe_connect(FeEnv* e, int align) {
     for (int which = 0; which < 2; ++which) { // _move_rotate_object(body, offset, [0,0,0]) incl. the step inside _is_inside
       LANES_BEGIN
         if (lane == 0) {
-          const int obj = which == 0 ? body1 : body2;
-          const int qa = m->link_qadr[m->nrlink + obj];
-          double tq[4] = {(double)w->qpos()[qa + 3], (double)w->qpos()[qa + 4], (double)w->qpos()[qa + 5], (double)w->qpos()[qa + 6]};
-          double tr[3] = {0, 0, -lift};
-          // note: _move_rotate_object does not stop the parts (no _stop_object call): keep velocities / gravcomp
-          const int g = fe_find(e->group, obj);
-          double base[7];
-          for (int k = 0; k < 7; ++k) base[k] = (double)w->qpos()[qa + k];
-          for (int i = 0; i < m->npart; ++i) {
-            if (fe_find(e->group, i) != g) continue;
-            const int qi = m->link_qadr[m->nrlink + i];
-            double q[7], np_[3], nq[4];
-            for (int k = 0; k < 7; ++k) q[k] = (double)w->qpos()[qi + k];
-            d_transform_to_target(base, q, tq, np_, nq);
-            for (int k = 0; k < 3; ++k) w->qpos()[qi + k] = (float)(np_[k] + tr[k]);
-            for (int k = 0; k < 4; ++k) w->qpos()[qi + 3 + k] = (float)nq[k];
-          }
+          const double tr[3] = {0, 0, -lift};
+          fe_move_group(e, which == 0 ? body1 : body2, tr, nullptr, false); // _move_rotate_object does not stop the parts
         }
       LANES_END
       fe_fwd_step(e);
@@ -586,9 +573,9 @@ FE_HD void fe_write_robot_ob(FeEnv* e, float* rb, int lane) {
 }
 
 // _get_obs under the flags of fe_set_obs_layout (furniture.py:1344-1387): the row [object_ob | subtask_ob | robot_ob | phase_ob], each entry present
-// as its flag asks, written to `ob` and, when `packed` is set, to that second row too.  It shows the subtask pair held in subtask_part, which the
-// step's dense reward has not moved yet.
-FE_FN void fe_write_obs_layout(FeEnv* e, float* ob, float* packed) {
+// as its flag asks, written to `ob` and, when `packed` is set, to that second row too.  The default flags give object_ob (7 per part, XML order)
+// then robot_ob (furniture_sawyer.py:103-155).  It shows the subtask pair held in subtask_part, which the step's dense reward has not moved yet.
+FE_FN void fe_write_obs(FeEnv* e, float* ob, float* packed) {
   FeWarp* w = e->w;
   const fe_model* m = w->m;
   const fe_scene* sc = e->sc;
@@ -611,27 +598,6 @@ FE_FN void fe_write_obs_layout(FeEnv* e, float* ob, float* packed) {
     }
     if (nsub && lane < 2) ob[nobj + lane] = (float)((lane == 0 ? p1 : p2) + 1); // [_subtask_part1 + 1, _subtask_part2 + 1] (:1379-1382)
     if (!(lay & FE_OBS_NO_ROBOT)) fe_write_robot_ob(e, ob + nobj + nsub, lane);
-    if (sc->phase_ob && lane < 8) ob[sc->obs_dim - 8 + lane] = (e->es.dstate && e->es.dstate[e->env].phase == lane) ? 1.f : 0.f;
-  LANES_END
-  }
-}
-
-// _get_obs: object_ob (7 per part, XML order) then robot_ob (furniture.py:1344-1387, furniture_sawyer.py:103-155), into the row `ob` and, when
-// `packed` is set, into that second row too; the other flags' rows are fe_write_obs_layout's
-FE_FN void fe_write_obs(FeEnv* e, float* ob, float* packed) {
-  FeWarp* w = e->w;
-  const fe_model* m = w->m;
-  const fe_scene* sc = e->sc;
-  if (sc->obs_layout) { fe_write_obs_layout(e, ob, packed); return; }
-  const int nrl = m->nrlink, np = m->npart;
-  for (int pass = 0; pass < (packed ? 2 : 1); ++pass) {
-  if (pass == 1) ob = packed;
-  LANES_BEGIN
-    for (int p = lane; p < np; p += 32) {
-      for (int k = 0; k < 3; ++k) ob[7 * p + k] = w->lpos()[3 * (nrl + p) + k];
-      for (int k = 0; k < 4; ++k) ob[7 * p + 3 + k] = w->lquat()[4 * (nrl + p) + k];
-    }
-    fe_write_robot_ob(e, ob + 7 * np, lane);
     if (sc->phase_ob && lane < 8) ob[sc->obs_dim - 8 + lane] = (e->es.dstate && e->es.dstate[e->env].phase == lane) ? 1.f : 0.f;
   LANES_END
   }
@@ -692,6 +658,25 @@ FE_FN void fe_env_preassemble_pair(FeEnv* e, int i) {
       for (int c = 0; c < sc->nconn; ++c) { if (sc->conn_site[c] == s1) e->si->conn1 = c; if (sc->conn_site[c] == s2) e->si->conn2 = c; }
     }
   LANES_END
+}
+
+// gravity compensation, this lane's share: qfrc_applied = qfrc_bias of the last forward pass on the arm and gripper dofs (furniture.py:3372-3377)
+FE_HD void fe_gravity_comp(FeEnv* e, int lane) {
+  FeWarp* w = e->w;
+  const fe_scene* sc = e->sc;
+  for (int i = lane; i < sc->narm; i += 32) w->qfrc_applied()[sc->arm_dof[i]] = w->bias()[sc->arm_dof[i]];
+  for (int i = lane; i < sc->ngrip; i += 32) w->qfrc_applied()[sc->grip_dof[i]] = w->bias()[sc->grip_dof[i]];
+}
+// the robot's collisions back on, this lane's share: the masks fe_env_reset_clear saved, or 0 under no_collision, whose saved masks are the
+// agent's zeros (furniture.py:1586-1595, :1962-1965)
+FE_HD void fe_restore_robot_masks(FeEnv* e, int lane) {
+  FeWarp* w = e->w;
+  const fe_model* m = w->m;
+  const int ng = m->ngeom;
+  const int* rct = e->es.robot_contype + (size_t)e->env * ng;
+  const int* rca = e->es.robot_conaff + (size_t)e->env * ng;
+  const bool off = e->es.no_collision[e->env] != 0;
+  for (int g = lane; g < ng; g += 32) if (m->geom_tag[g] & FE_TAG_ROBOT) { w->contype()[g] = off ? 0 : rct[g]; w->conaff()[g] = off ? 0 : rca[g]; }
 }
 
 // FurnitureEnv._reset (furniture.py:1406-1663) in non-inlined parts called one after the other by fe_env_reset_one, so that the connect path of
@@ -804,21 +789,11 @@ FE_FN void fe_env_reset_place(FeEnv* e) {
 }
 // gravity compensation and 101 robot poses, the second one with the robot's collisions back on (:1569-1612)
 FE_FN void fe_env_reset_robot(FeEnv* e) {
-  FeWarp* w = e->w;
-  const fe_model* m = w->m;
-  const fe_scene* sc = e->sc;
-  const int ng = m->ngeom;
-  const int* rct = e->es.robot_contype + (size_t)e->env * ng;
-  const int* rca = e->es.robot_conaff + (size_t)e->env * ng;
-  const bool off = e->es.no_collision[e->env] != 0; // the masks the reset saved are the agent's zeros (furniture.py:1962-1965)
   // gravity compensation, robot pose, one step with robot collisions still off (furniture.py:1569-1584)
   for (int phase = 0; phase < 101; ++phase) {
     LANES_BEGIN
-      if (phase <= 1) {
-        for (int i = lane; i < sc->narm; i += 32) w->qfrc_applied()[sc->arm_dof[i]] = w->bias()[sc->arm_dof[i]];
-        for (int i = lane; i < sc->ngrip; i += 32) w->qfrc_applied()[sc->grip_dof[i]] = w->bias()[sc->grip_dof[i]];
-      }
-      if (phase == 1) for (int g = lane; g < ng; g += 32) if (m->geom_tag[g] & FE_TAG_ROBOT) { w->contype()[g] = off ? 0 : rct[g]; w->conaff()[g] = off ? 0 : rca[g]; } // :1586-1595
+      if (phase <= 1) fe_gravity_comp(e, lane);
+      if (phase == 1) fe_restore_robot_masks(e, lane); // :1586-1595
       if (lane == 0) fe_init_robot_pos(e);
     LANES_END
     fe_fwd_step(e);
@@ -838,10 +813,7 @@ FE_FN void fe_env_reset_sync(FeEnv* e, int pre) {
     for (int i = lane; i < m->nv; i += 32) w->warm()[i] = 0.f;
   LANES_END
   fe_forward(e->w);
-  LANES_BEGIN
-    for (int i = lane; i < sc->narm; i += 32) w->qfrc_applied()[sc->arm_dof[i]] = w->bias()[sc->arm_dof[i]];
-    for (int i = lane; i < sc->ngrip; i += 32) w->qfrc_applied()[sc->grip_dof[i]] = w->bias()[sc->grip_dof[i]];
-  LANES_END
+  LANES_BEGIN fe_gravity_comp(e, lane); LANES_END
   for (int i = 0; i < 100; ++i) fe_fwd_step(e);
   LANES_BEGIN
     if (lane == 0) {
@@ -862,10 +834,6 @@ FE_FN void fe_env_reset_sync(FeEnv* e, int pre) {
 FE_FN void fe_env_set_init_state(FeEnv* e, int s, bool robot) {
   FeWarp* w = e->w;
   const fe_model* m = w->m;
-  const int ng = m->ngeom;
-  const int* rct = e->es.robot_contype + (size_t)e->env * ng;
-  const int* rca = e->es.robot_conaff + (size_t)e->env * ng;
-  const bool off = e->es.no_collision[e->env] != 0;
   const float* q = e->es.init_qpos + (size_t)s * m->nq;
   const float* v = e->es.init_qvel + (size_t)s * m->nv;
   LANES_BEGIN
@@ -873,7 +841,7 @@ FE_FN void fe_env_set_init_state(FeEnv* e, int s, bool robot) {
     for (int i = lane; i < m->nq; i += 32) w->qpos()[i] = q[i];
     for (int i = lane; i < m->nv; i += 32) w->qvel()[i] = v[i];
     for (int i = lane; i < m->nu; i += 32) w->ctrl()[i] = 0.f;
-    if (robot) for (int g = lane; g < ng; g += 32) if (m->geom_tag[g] & FE_TAG_ROBOT) { w->contype()[g] = off ? 0 : rct[g]; w->conaff()[g] = off ? 0 : rca[g]; }
+    if (robot) fe_restore_robot_masks(e, lane);
   LANES_END
 }
 // the pick before every reset (furniture.py:1433-1434): `if np.random.rand() > 0.2: set_init_qpos(np.random.choice(states))` over the first
@@ -953,8 +921,7 @@ FE_HD void fe_env_controls(FeEnv* e, const float* a, float grip) {
       }
       w->ctrl()[u] = v;
     }
-    for (int i = lane; i < sc->narm; i += 32) w->qfrc_applied()[sc->arm_dof[i]] = w->bias()[sc->arm_dof[i]]; // gravity compensation, :3372-3377
-    for (int i = lane; i < sc->ngrip; i += 32) w->qfrc_applied()[sc->grip_dof[i]] = w->bias()[sc->grip_dof[i]];
+    fe_gravity_comp(e, lane);
     if (lane == 0) fe_env_clear_flags(e);
   LANES_END
 }
@@ -972,9 +939,8 @@ FE_HD void fe_env_finish(FeEnv* e, const float* a, int act_dim, float connect, i
   } else {
     if (connect > 0.f) { // furniture.py:1290-1322: per arm, the first part both of its fingers touch; stop at the first connection
       for (int arm = 0; arm < sc->narms; ++arm) {
-        const int both = arm == 0 ? 3 : 24;
         int part = -1;
-        for (int p = 0; p < np; ++p) if ((w->touch()[p] & both) == both) { part = p; break; }
+        for (int p = 0; p < np; ++p) if (fe_both_fingers(w->touch()[p], arm)) { part = p; break; }
         if (part >= 0) {
           fe_try_connect_scan(e, part);
           if (e->si->aligned) { fe_connect(e, FE_ALIGN_CONFIG); break; }
@@ -988,7 +954,7 @@ FE_HD void fe_env_finish(FeEnv* e, const float* a, int act_dim, float connect, i
         if (lane == 0) {
           const int b1 = e->si->repin, qa = m->link_qadr[m->nrlink + b1];
           double tr[3] = {e->sd->body1_pose[0] - (double)w->qpos()[qa], e->sd->body1_pose[1] - (double)w->qpos()[qa + 1], e->sd->body1_pose[2] - (double)w->qpos()[qa + 2]};
-          fe_move_group(e, b1, tr, e->sd->body1_pose + 3, 0.f);
+          fe_move_group(e, b1, tr, e->sd->body1_pose + 3, true);
           e->si->repin = -1;
         }
       LANES_END
@@ -1008,8 +974,8 @@ FE_HD void fe_env_finish(FeEnv* e, const float* a, int act_dim, float connect, i
       if (!fail)
         for (int arm = 0; arm < sc->narms; ++arm) // furniture.py:492-523: both fingers of the same arm
           for (int p = 0; p < np; ++p) {
-            const int t = w->touch()[p], both = arm == 0 ? 3 : 24;
-            if ((t & both) == both) {
+            const int t = w->touch()[p];
+            if (fe_both_fingers(t, arm)) {
               if (!touched[p]) { touched[p] = 1; touch_r += coef[1]; }
               if (!(t & 4) && !picked[p]) { picked[p] = 1; pick_r += coef[2]; }
             }
@@ -1083,10 +1049,7 @@ FE_FN void fe_env_step_one(FeEnv* e, const float* action, float* reward_out, uin
   const float connect = a[sc->connect_action_index];
   fe_env_controls(e, a, grip);
   fe_env_agent_masks(e);
-  const int n = e->es.substeps[e->env];
-  for (int i = 0; fe_block_any(i < n); ++i) { // _do_simulation, furniture.py:2877-2879
-    if (i < n) fe_substep_lockstep(w); else fe_substep_idle();
-  }
+  fe_substeps_mixed(w, e->es.substeps[e->env]); // _do_simulation, furniture.py:2877-2879
   const int fail = (w->u()[FE_U_FLAGS] & FE_FLAG_DIVERGED) ? 1 : 0; // MujocoException path, :2889-2897
   fe_env_finish(e, a, sc->act_dim, connect, fail, fail, reward_out, done_out, info_out);
 }

@@ -230,9 +230,7 @@ FE_FN void fe_env_ik_step_one(FeEnv* e, FeIkArgs ik, const float* action, float*
       LANES_END
     }
     fe_env_controls(e, st->low, grip);
-    for (int i = 0; fe_block_any(i < n); ++i) {
-      if (i < n) fe_substep_lockstep(w); else fe_substep_idle();
-    }
+    fe_substeps_mixed(w, n);
     if (w->u()[FE_U_FLAGS] & FE_FLAG_DIVERGED) { // _do_simulation's except branch: reset, then the remaining repeats run on the new episode (furniture.py:2889-2897)
       fail = 1;
       FE_SYNC;

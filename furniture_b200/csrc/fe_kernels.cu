@@ -19,32 +19,32 @@ extern "C" __global__ void __launch_bounds__(32 * FE_MAX_WPB) fe_sim_kernel(FeSt
   fe_run_env(s, m, opt, env, nsub, mode, fe_smem + (size_t)wib * slice_words, dbg);
 }
 
-// the step kernels, one per control type: same launch shape, envs packed into blocks by fe_order_kernel
+// the step kernels, one per control type: same launch shape, envs packed into blocks by fe_order_kernel.  The warp's slot names its env
+// in `slots`; an unused slot (blocks of heavy envs are deliberately left partly empty) returns at once.  Then `step(FeEnv*)` in the env's slice
+template <class Step>
+__device__ __forceinline__ void fe_env_step_slot(const FeState& st, const FeEnvState& es, const fe_model* m, const fe_scene* sc, const fe_config* cfg,
+                                                 const FeOpt& opt, int slice_words, const int* slots, Step step) {
+  const int wib = threadIdx.x >> 5, env = slots[blockIdx.x * (blockDim.x >> 5) + wib];
+  if (env < 0) return;
+  fe_env_run(fe_smem + (size_t)wib * (slice_words + FE_ENV_EXTRA_WORDS), m, sc, cfg, opt, st, es, env, slice_words, step);
+}
+
 extern "C" __global__ void __launch_bounds__(32 * FE_MAX_WPB) fe_env_step_kernel(FeState st, FeEnvState es, const fe_model* __restrict__ m, const fe_scene* __restrict__ sc,
                                                          fe_config cfg, FeOpt opt, const float* __restrict__ actions, float* reward, uint8_t* done,
                                                          int32_t* info, int slice_words, const int* __restrict__ slots) {
-  const int wib = threadIdx.x >> 5, slot = blockIdx.x * (blockDim.x >> 5) + wib;
-  const int env = slots[slot];
-  if (env < 0) return; // unused slot (blocks of heavy envs are deliberately left partly empty)
-  fe_env_run(fe_smem + (size_t)wib * (slice_words + FE_ENV_EXTRA_WORDS), m, sc, &cfg, opt, st, es, env, slice_words, [&](FeEnv* e) { fe_env_step_one(e, actions, reward, done, info); });
+  fe_env_step_slot(st, es, m, sc, &cfg, opt, slice_words, slots, [&](FeEnv* e) { fe_env_step_one(e, actions, reward, done, info); });
 }
 
 extern "C" __global__ void __launch_bounds__(32 * FE_MAX_WPB) fe_env_ik_step_kernel(FeState st, FeEnvState es, FeIkArgs ik, const fe_model* __restrict__ m,
                                                             const fe_scene* __restrict__ sc, fe_config cfg, FeOpt opt, const float* __restrict__ actions,
                                                             float* reward, uint8_t* done, int32_t* info, int slice_words, const int* __restrict__ slots) {
-  const int wib = threadIdx.x >> 5, slot = blockIdx.x * (blockDim.x >> 5) + wib;
-  const int env = slots[slot];
-  if (env < 0) return; // unused slot (blocks of heavy envs are deliberately left partly empty)
-  fe_env_run(fe_smem + (size_t)wib * (slice_words + FE_ENV_EXTRA_WORDS), m, sc, &cfg, opt, st, es, env, slice_words, [&](FeEnv* e) { fe_env_ik_step_one(e, ik, actions, reward, done, info); });
+  fe_env_step_slot(st, es, m, sc, &cfg, opt, slice_words, slots, [&](FeEnv* e) { fe_env_ik_step_one(e, ik, actions, reward, done, info); });
 }
 
 extern "C" __global__ void __launch_bounds__(32 * FE_MAX_WPB) fe_env_ctl_step_kernel(FeState st, FeEnvState es, FeCtlArgs ctl, const fe_model* __restrict__ m,
                                                              const fe_scene* __restrict__ sc, fe_config cfg, FeOpt opt, const float* __restrict__ actions,
                                                              float* reward, uint8_t* done, int32_t* info, int slice_words, const int* __restrict__ slots) {
-  const int wib = threadIdx.x >> 5, slot = blockIdx.x * (blockDim.x >> 5) + wib;
-  const int env = slots[slot];
-  if (env < 0) return; // unused slot (blocks of heavy envs are deliberately left partly empty)
-  fe_env_run(fe_smem + (size_t)wib * (slice_words + FE_ENV_EXTRA_WORDS), m, sc, &cfg, opt, st, es, env, slice_words, [&](FeEnv* e) { fe_env_ctl_step_one(e, ctl, actions, reward, done, info); });
+  fe_env_step_slot(st, es, m, sc, &cfg, opt, slice_words, slots, [&](FeEnv* e) { fe_env_ctl_step_one(e, ctl, actions, reward, done, info); });
 }
 
 extern "C" __global__ void __launch_bounds__(32 * FE_MAX_WPB) fe_env_reset_kernel(FeState st, FeEnvState es, const fe_model* __restrict__ m, const fe_scene* __restrict__ sc,
