@@ -47,7 +47,7 @@ FE_HDN void fe_dense_begin_subtask(const W& w, const fe_dense_config* c, const f
   } else {
     st->phase = FE_PH_ABOVE_LEG;
   }
-  if (c->diff_rew) {
+  if (st->diff_rew) {
     if (st->phase == FE_PH_ABOVE_LEG) {
       double g[3];
       fe_dense_grasp(w, rc, s, g, (double*)nullptr);
@@ -68,16 +68,17 @@ template <class W>
 FE_HDN void fe_dense_begin_episode(const W& w, const fe_dense_config* c, const fe_dense_recipe* rc, int first, FeDenseState* st) {
   st->subtask = first;
   st->success = 0;
+  st->diff_rew = c->diff_rew; // the shaped terms keep their prev[] slots only in diff mode: the mode holds for the whole episode
   for (int k = 0; k < FE_DP_N; ++k) st->prev[k] = 0.0;
   st->prev[FE_DP_GRASP] = -1.0;
   for (int k = 0; k < 3; ++k) st->init_eef[k] = 0.0;
   fe_dense_begin_subtask(w, c, rc, st);
 }
 
-// shaped term of a quantity x with memory: diff_rew -> coef * mult * (f(x) - f(prev)) (or the reverse), prev := x; else the plain term
+// shaped term of a quantity x with memory: diff_rew (the episode's) -> coef * mult * (f(x) - f(prev)) (or the reverse), prev := x; else the plain term
 #define FE_DENSE_SHAPED(out, slot, x, coef, mult, FEXPR, reversed, plain)            \
   do {                                                                               \
-    if (c->diff_rew) {                                                               \
+    if (st->diff_rew) {                                                              \
       double v_ = (x);            const double cur_ = (FEXPR);                       \
       v_ = st->prev[slot];        const double old_ = (FEXPR);                       \
       out = ndmul(ndmul((reversed) ? ndsub(old_, cur_) : ndsub(cur_, old_), (coef)), (mult)); \

@@ -22,7 +22,8 @@ enum { FE_DP_INIT_EEF, FE_DP_ABOVE_LEG, FE_DP_EEF_LEG, FE_DP_GRASP, FE_DP_LIFT_Z
 enum { FE_PH_INIT_EEF, FE_PH_ABOVE_LEG, FE_PH_LOWER_EEF, FE_PH_GRASP, FE_PH_LIFT, FE_PH_ALIGN, FE_PH_MOVE, FE_PH_FINE };
 
 struct FeDenseState { // per env, in HBM; lane 0 reads and writes it once per step
-  int32_t phase, subtask, dropped, table_moved, lifted, fine_aligned, success, pad_;
+  int32_t phase, subtask, dropped, table_moved, lifted, fine_aligned, success;
+  int32_t diff_rew; // fe_dense_config.diff_rew of the env's row at the start of the episode
   double table_site0[3], leg0[3], lift_target[3], init_eef[3];
   double prev[FE_DP_N];
 };

@@ -85,7 +85,7 @@ struct FeEnvState {
   int *robot_contype, *robot_conaff;           // [N][ngeom] saved robot masks during reset
   float* episode_reward;
   // dense (phase-based) reward, fe_dense.h: NULL = the sparse reward of FurnitureEnv._compute_reward
-  const fe_dense_config* dense;
+  const fe_dense_config* dense;                // [N] each env's coefficients and flags; lane 0 reads its row once per step
   FeDenseState* dstate;                        // [N]
   float* dinfo;                                // [N][FE_DENSE_INFO]
 };
@@ -822,7 +822,7 @@ FE_FN void fe_env_reset_sync(FeEnv* e, int pre) {
       fe_next_subtask(e); // :1653, after the preassembly in both branches
       if (e->es.dense) { // FurnitureSawyerDenseRewardEnv._reset: _reset_reward_variables on the settled scene
         FeSliceWorld world = {w};
-        fe_dense_begin_episode(world, e->es.dense, &sc->dense, pre, e->es.dstate + e->env); // dense_info keeps the last step's terms (the terminal step's, after an auto-reset)
+        fe_dense_begin_episode(world, e->es.dense + e->env, &sc->dense, pre, e->es.dstate + e->env); // dense_info keeps the last step's terms (the terminal step's, after an auto-reset)
         fe_dense_subtask_pair(e, pre);
       }
     }
@@ -1000,7 +1000,7 @@ FE_HD void fe_env_finish(FeEnv* e, const float* a, int act_dim, float connect, i
         int dd = 0;
         FeDenseState* ds = e->es.dstate + env;
         const int sub0 = ds->subtask;
-        fe_dense_step(world, e->es.dense, &sc->dense, thr, n_goal, ds, ad, act_dim, connected_now, &dr, &dd, di);
+        fe_dense_step(world, e->es.dense + e->env, &sc->dense, thr, n_goal, ds, ad, act_dim, connected_now, &dr, &dd, di);
         e->si->dense_pair = ds->subtask != sub0 && !ds->success; // _set_next_subtask moved on without finishing (furniture_sawyer_dense.py:141-147)
         reward = (float)dr;
         success = ds->success;

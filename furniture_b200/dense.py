@@ -24,6 +24,8 @@ _COEFS = ["phase_bonus", "ctrl_penalty_coef", "eef_forward_dist_coef", "eef_up_d
           "align_pos_threshold", "align_rot_threshold", "move_pos_dist_coef", "move_rot_dist_coef", "move_pos_threshold", "move_rot_threshold",
           "move_fine_pos_exp_coef", "move_fine_pos_dist_coef", "move_fine_rot_dist_coef", "aligned_bonus_coef"]
 _FLAGS = ["diff_rew", "early_termination", "phase_ob", "reset_robot_after_attach"]
+# what each env of a dense handle may hold on its own (Engine.set_dense_options): everything but phase_ob, which sets the obs width
+PER_ENV_KEYS = tuple(_COEFS) + ("diff_rew", "early_termination", "reset_robot_after_attach")
 
 DENSE_DEFAULTS = dict(
     diff_rew=True, early_termination=False, phase_ob=False, reset_robot_after_attach=False,

@@ -14,7 +14,7 @@ import os
 import numpy as np
 
 from . import mjcf
-from .dense import FeDenseConfig, FeDenseRecipe, dense_config, pack_dense_recipe
+from .dense import PER_ENV_KEYS as DENSE_KEYS, FeDenseConfig, FeDenseRecipe, dense_config, pack_dense_recipe
 from .engine_model import MAXEQ, MAXPART, MAXRDOF, MAXSITE, MAXU, EngineModel
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -44,6 +44,9 @@ OPTIONS = dict(
     furn_rot_rand=("placement_rand", 1, None), agent_xyz_rand=("placement_rand", 2, None), success_reward=("reward_coef", 0, None),
     touch_reward=("reward_coef", 1, None), pick_reward=("reward_coef", 2, None), ctrl_penalty_coef=("reward_coef", 3, None),
     unstable_penalty_coef=("reward_coef", 4, None), max_episode_steps=("max_episode_steps", 0, None))
+# the dense reward's per-env options (config/furniture_sawyer_dense.py:23-70): members of each env's fe_dense_config row, field dense_config;
+# Engine.set_dense_options writes them through the same path.  Two keys share a name with an OPTIONS key, hence a table of their own.
+DENSE_OPTIONS = {k: ("dense_config", k, None) for k in DENSE_KEYS}
 
 
 class FeConfig(C.Structure):
@@ -378,9 +381,29 @@ class Engine:
             raise ValueError("unknown task options %s (known: %s)" % (unknown, sorted(TASK_OPTIONS)))
         self._set_options(envs, values)
 
-    def _set_options(self, envs, values):
-        """writes `values` (OPTIONS keys -> a scalar or one value per env of `envs`; None leaves an option as it is) for the envs in `envs`
-        (default: all).  Every value is checked and converted before any field is written, and each field touched is written once."""
+    def set_dense_options(self, envs=None, **values):
+        """the dense reward's coefficients, thresholds (config/furniture_sawyer_dense.py:23-70, ctrl_penalty_coef included), diff_rew,
+        early_termination and reset_robot_after_attach for the envs in `envs` (default: all), each a scalar or one value per env of
+        `envs`, so that one batch can run a sweep or a curriculum over them.  They act from the env's next step; diff_rew from its next
+        reset, since an episode's shaped terms difference against what they kept in its mode; reset_robot_after_attach, which the arm follows
+        too, from its next connection.  phase_ob sets the obs width and stays the handle's."""
+        if self.model.meta.get("agent") == "Cursor":
+            raise ValueError("the Cursor env's reward is host code (cursor_env.FurnitureCursorEnvB200); it has no dense reward")
+        if self.dense is None:
+            raise ValueError("this handle runs the sparse reward: the dense options need a handle built with the dense reward")
+        unknown = sorted(set(values) - set(DENSE_OPTIONS))
+        if unknown:
+            raise ValueError("unknown dense options %s (known: %s; phase_ob is one per handle)" % (unknown, sorted(DENSE_OPTIONS)))
+        self._set_options(envs, values, DENSE_OPTIONS)
+
+    def dense_rows(self):
+        """(N,) record array of every env's fe_dense_config row (a host copy of field dense_config)"""
+        return self.get("dense_config")[:, 0].view(np.dtype(FeDenseConfig))
+
+    def _set_options(self, envs, values, table=OPTIONS):
+        """writes `values` (keys of `table` -> a scalar or one value per env of `envs`; None leaves an option as it is) for the envs in `envs`
+        (default: all).  A column is an index into the field's row, or the name of a member of its struct-valued row.  Every value is
+        checked and converted before any field is written, and each field touched is written once."""
         idx = np.arange(self.N) if envs is None else np.asarray(envs, dtype=np.int64).ravel()
         if idx.size and (idx.min() < 0 or idx.max() >= self.N):
             raise IndexError("envs must lie in [0, %d), got %s" % (self.N, idx.tolist()))
@@ -388,7 +411,7 @@ class Engine:
         for key, v in values.items():
             if v is None:
                 continue
-            name, col, convert = OPTIONS[key]
+            name, col, convert = table[key]
             v = np.asarray(v if convert is None else convert(self, v))
             if v.ndim > 1 or (v.ndim == 1 and v.shape != idx.shape):
                 raise ValueError("%s takes a scalar or one value per env of `envs` (%d), got shape %s" % (key, idx.size, v.shape))
@@ -396,7 +419,11 @@ class Engine:
         for name, cols in columns.items():
             cur = self.get(name)
             for col, v in cols:
-                cur[idx, col] = v.astype(cur.dtype)
+                if isinstance(col, str):
+                    rows = cur[:, 0].view(np.dtype(FeDenseConfig))  # a view: writing its member writes `cur`
+                    rows[col][idx] = v.astype(rows.dtype[col])
+                else:
+                    cur[idx, col] = v.astype(cur.dtype)
             self.set(name, cur)
 
     def close(self):

@@ -126,11 +126,12 @@ def split_dense_config(config):
     cfg = dict(vars(config)) if hasattr(config, "__dict__") and not isinstance(config, dict) else dict(config or {})
     merged = dict(DENSE_ENV_DEFAULTS)
     merged.update({k: v for k, v in cfg.items() if v is not None})
-    name, over, ignored = split_config(merged)
-    over.pop("reset_robot_after_attach", None)  # the dense reward's flag drives both its phase machine and the arm
-    dense = {k: merged[k] for k in DENSE_DEFAULTS if k in merged}
+    name, over, ignored = split_config({k: v for k, v in merged.items() if k != "reset_robot_after_attach"})
+    dense = {k: merged[k] for k in DENSE_DEFAULTS if k in merged}  # a list gives one value per env (Engine.set_dense_options)
     if "ctrl_penalty_coef" in over:
         dense["ctrl_penalty_coef"] = over["ctrl_penalty_coef"]
+        if np.ndim(over["ctrl_penalty_coef"]) > 0:  # per env it is the phase machine's only: FeConfig keeps the default
+            del over["ctrl_penalty_coef"]
     return name, over, dense, [k for k in ignored if k not in DENSE_DEFAULTS]
 
 
@@ -163,7 +164,8 @@ def build_engine(agent, furniture_name, num_envs, device=0, lib_path=None, dense
                  **cfg_overrides):
     """The Engine of `num_envs` envs of `agent` + `furniture_name` that both env surfaces run; `lib_path` as for Engine.  The keywords:
         `dense`: None for the sparse reward of FurnitureEnv; a dict of coefficient overrides (possibly empty) for the phase-based
-        reward of FurnitureSawyerDenseRewardEnv, computed inside the step kernel (furniture_b200/dense.py).
+        reward of FurnitureSawyerDenseRewardEnv, computed inside the step kernel (furniture_b200/dense.py).  A sequence gives one value per
+        env (see Engine.set_dense_options; phase_ob is one per handle), the handle-wide config keeping the default.
         `control_type`: "impedance" (joint velocities, dof 9), "ik" (move 3, rotate 3, gripper, connect: dof 8) or "ik_quaternion" (the
         rotation as a quaternion relative to the hand: dof 9); the inverse kinematics and its three closed-loop repeats run inside the
         step kernel (furniture_b200/ik.py); or one of the NEW_CONTROLLERS ("position", "position_orientation", "joint_impedance",
@@ -217,7 +219,9 @@ def build_engine(agent, furniture_name, num_envs, device=0, lib_path=None, dense
 
         ctl_cfg = ctl_config(control_type, model=model, move_speed=(ik or {}).get("move_speed", 0.1))
     obs_flags = dict(robot_ob=bool(robot_ob), object_ob=bool(object_ob), object_ob_all=bool(object_ob_all), subtask_ob=bool(subtask_ob))
-    engine = Engine(model, num_envs, device=device, config=cfg, lib_path=lib_path, dense=dense_config(**dense) if dense is not None else None,
+    dense_per_env = {k: v for k, v in (dense or {}).items() if np.ndim(v) > 0}
+    dense_cfg = dense_config(**{k: v for k, v in dense.items() if k not in dense_per_env}) if dense is not None else None
+    engine = Engine(model, num_envs, device=device, config=cfg, lib_path=lib_path, dense=dense_cfg,
                     ik=ik_cfg, controller=ctl_cfg, obs_layout=obs_flags, fix_init=fix_init, fix_init_parts=fix_init_parts,
                     reset_robot_after_attach=reset_robot_after_attach, assembled=assembled)
     engine.control_type, engine.resize_factor = control_type, resize_factor
@@ -225,6 +229,8 @@ def build_engine(agent, furniture_name, num_envs, device=0, lib_path=None, dense
         engine.set_sim_options(control_freq=control_freq, no_collision=no_collision if np.any(no_collision) else None)
     if per_env:
         engine.set_task_options(**per_env)
+    if dense_per_env:  # a reset_robot_after_attach among them sets the arm's flag of each env too
+        engine.set_dense_options(**dense_per_env)
     if prefix_length(preassembled) or num_connects is not None:
         engine.set_subtask(prefix_length(preassembled), num_connects)
     apply_init_config(engine, load_init_states, load_demo)
@@ -297,6 +303,12 @@ class BatchedFurnitureEnv:
         noise, the reward coefficients and max_episode_steps of config/furniture.py by their key names (Engine.set_task_options), so that
         one batch can run a curriculum over them"""
         self.engine.set_task_options(envs, **values)
+
+    def set_dense_options(self, envs=None, **values):
+        """per env (`envs`, default: all; a scalar or one value per env of `envs`): the dense reward's coefficients, thresholds, diff_rew,
+        early_termination and reset_robot_after_attach by the names of config/furniture_sawyer_dense.py (Engine.set_dense_options), so that
+        one batch can run a reward sweep or a threshold curriculum"""
+        self.engine.set_dense_options(envs, **values)
 
     def set_subtask(self, subtask, num_connects=None):
         """FurnitureEnv.set_subtask (furniture.py:204-207) with a scalar or an (N,) array each, so that the envs of one batch can train different
@@ -469,6 +481,11 @@ class MixedFurnitureEnv:
         """BatchedFurnitureEnv.set_task_options with `envs` as global indices of this batch (default: all); each value is a scalar or one
         per env of `envs`"""
         self._per_bucket(envs, values, lambda b, idx, v: b.set_task_options(idx, **v))
+
+    def set_dense_options(self, envs=None, **values):
+        """BatchedFurnitureEnv.set_dense_options with `envs` as global indices of this batch (default: all); each value is a scalar or one
+        per env of `envs`"""
+        self._per_bucket(envs, values, lambda b, idx, v: b.set_dense_options(idx, **v))
 
     def _per_bucket(self, envs, values, set_options):
         """set_options(bucket, its envs, their values) for every bucket that holds some of `envs` (global indices, default: all), each of

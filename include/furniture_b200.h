@@ -127,11 +127,17 @@ int fe_sim_step(fe_handle* h, int nsub, void* stream);
    step; placement_rand (3 x float32 per env, read/write: furn_xyz_rand, furn_rot_rand, agent_xyz_rand, :177-194), from the env's next reset,
    agent_xyz_rand also from its next connection under reset_robot_after_attach; reward_coef (5 x float32 per env, read/write: success_reward,
    touch_reward, pick_reward, ctrl_penalty_coef, unstable_penalty_coef, :291-295), from the env's next step; max_episode_steps (int32, one
-   per env, read/write: :163-168), at once, an episode ending when its length equals it (fe_set_max_episode_steps writes every env's).
+   per env, read/write: :163-168), at once, an episode ending when its length equals it (fe_set_max_episode_steps writes every env's);
+   dense_config (one fe_dense_config per env, typestr "|V" + its size, read/write, a dense handle only: fe_enable_dense_reward fills every
+   row with its argument): the env's coefficients, thresholds and flags of the dense reward, from its next step, but diff_rew, which an
+   episode keeps from its start (the shaped terms difference against values kept in that mode only).  Writing it sets every env's
+   reset_robot_after_attach from its row.  fe_set_field refuses rows whose struct_bytes is not sizeof(fe_dense_config), whose diff_rew,
+   early_termination or reset_robot_after_attach is outside {0, 1}, whose phase_ob disagrees with the handle's (the obs width is the
+   handle's) or that hold a non-finite coefficient or threshold.
    fe_set_field refuses flags outside {0, 1}, substeps below 1, fix_init_parts bits at or beyond the
    number of parts, non-finite fix_pose values or zero quaternions, fix_have = 1 for an env whose fix_pose was never written, non-finite
    alignment / placement_rand / reward_coef values, max_episode_steps below 1 and, in a dense handle, a reset_robot_after_attach that
-   differs from the dense reward's or a reward_coef whose first four columns differ from the handle's fe_config (the phase machine
+   differs from the env's dense_config row or a reward_coef whose first four columns differ from the handle's fe_config (the phase machine
    replaces those terms; its ctrl_penalty_coef is fe_dense_config's) */
 int fe_get_field(fe_handle* h, const char* name, void* dst_host, size_t bytes);
 int fe_set_field(fe_handle* h, const char* name, const void* src_host, size_t bytes);
@@ -211,7 +217,7 @@ int fe_env_step_host(fe_handle* h, const float* actions_host, float* obs_host, f
    every env's field max_episode_steps and the handle's fe_config; takes effect from the next step */
 int fe_set_max_episode_steps(fe_handle* h, int max_episode_steps);
 /* Switch the handle to the dense reward; call before the first fe_env_reset.  The scene must carry a recipe, and dc->phase_ob must agree
- * with the scene (the one-hot phase is part of obs_dim).  fe_env_step then returns the dense reward / done / success, and field
+ * with the scene (the one-hot phase is part of obs_dim).  Every env's row of field "dense_config" starts as dc (see fe_set_field).  fe_env_step then returns the dense reward / done / success, and field
  * "dense_info" holds (n_envs, fe_dense_info_dim()) float32 per step: phase, subtask, phase_bonus, ctrl_penalty, gripper_penalty,
  * move_other_part_penalty, drop_penalty, touch, drop_leg, table_moved, stable_grip_succ, skips (bit 0 to lift_leg, bit 1 to move_leg_fine). */
 int fe_enable_dense_reward(fe_handle* h, const fe_dense_config* dc);

@@ -63,34 +63,57 @@ class World:
         return self.leg_pos[s] + self.leg_R[s][:, 0] * 0.02
 
 
-def main():
+def reference_dense_env():
+    """the reference's FurnitureSawyerDenseRewardEnv class with its parent constructor stubbed (no simulator), and its default config"""
     T, FurnitureEnv = import_reference()
     from furniture.env.furniture_sawyer import FurnitureSawyerEnv
     from furniture.env.furniture_sawyer_dense import FurnitureSawyerDenseRewardEnv as Dense
     from furniture.config import create_parser
-    from furniture.env.models import furniture_name2id
 
     argv, sys.argv = sys.argv, sys.argv[:1]
     base_cfg = create_parser("IKEASawyerDense-v0").parse_args([])
     sys.argv = argv
     FurnitureSawyerEnv.__init__ = lambda self, config: None  # no simulator: only the dense env's own attribute set-up runs
+    return Dense, FurnitureEnv, base_cfg
 
-    rng = np.random.RandomState(20260924)
-    rec = {k: [] for k in ("episode", "is_reset", "leg_pos", "leg_site_pos", "leg_site_mat", "table_site_pos", "table_site_mat", "gl", "gr", "touchL",
-                           "touchR", "eef", "grip_mat", "connected", "ac", "reward", "done", "success", "phase", "subtask", "info")}
-    eps = {k: [] for k in ("recipe", "diff_rew", "early_termination", "phase_ob", "reset_robot_after_attach", "nsub")}
-    coef_names = None
-    recipe_json = {}
-    n_ep = 0
-    branch = {}
-    while len(rec["reward"]) < 9000:
-        recipe_name = RECIPES[n_ep % len(RECIPES)]
-        cfg = types.SimpleNamespace(**vars(base_cfg))
-        cfg.furniture_name = recipe_name
-        cfg.diff_rew = bool(rng.rand() < 0.7)
-        cfg.early_termination = bool(rng.rand() < 0.4)
-        cfg.phase_ob = bool(rng.rand() < 0.25)
-        cfg.reset_robot_after_attach = bool(rng.rand() < 0.3)
+
+def draw_flags(rng, cfg):
+    """the three flags and phase_ob of an episode"""
+    cfg.diff_rew = bool(rng.rand() < 0.7)
+    cfg.early_termination = bool(rng.rand() < 0.4)
+    cfg.phase_ob = bool(rng.rand() < 0.25)
+    cfg.reset_robot_after_attach = bool(rng.rand() < 0.3)
+
+
+class Recorder:
+    """runs scripted episodes of the reference's dense env and keeps what it showed and what the reference answered"""
+
+    def __init__(self):
+        self.Dense, self.FurnitureEnv, self.base_cfg = reference_dense_env()
+        self.rec = {k: [] for k in ("episode", "is_reset", "leg_pos", "leg_site_pos", "leg_site_mat", "table_site_pos", "table_site_mat", "gl", "gr",
+                                    "touchL", "touchR", "eef", "grip_mat", "connected", "ac", "reward", "done", "success", "phase", "subtask", "info")}
+        self.eps = {k: [] for k in ("recipe", "diff_rew", "early_termination", "phase_ob", "reset_robot_after_attach", "nsub")}
+        self.recipe_json = {}
+        self.branch = {}
+        self.n_ep = 0
+        cfg = self.base_cfg
+        self.coef_names = sorted(k for k, v in vars(cfg).items() if isinstance(v, (int, float, bool)) and ("coef" in k or "threshold" in k or k in (
+            "phase_bonus", "alignment_pos_dist", "alignment_rot_dist_up", "alignment_rot_dist_forward", "alignment_project_dist")))
+
+    def new_config(self, rng, configure=draw_flags):
+        """the next episode's config: the reference's defaults for the next recipe, then `configure(rng, cfg)`"""
+        cfg = types.SimpleNamespace(**vars(self.base_cfg))
+        cfg.furniture_name = RECIPES[self.n_ep % len(RECIPES)]
+        configure(rng, cfg)
+        return cfg
+
+    def episode(self, rng, cfg, record=True):
+        """one scripted episode under `cfg`; with record=False nothing is kept and the episode's phase trace is returned"""
+        from furniture.env.models import furniture_name2id
+
+        Dense, FurnitureEnv = self.Dense, self.FurnitureEnv
+        rec = self.rec if record else {k: [] for k in self.rec}
+        recipe_name = cfg.furniture_name
         env = object.__new__(Dense)
         Dense.__init__(env, cfg)
         env._config = cfg
@@ -103,7 +126,7 @@ def main():
         S = len(env._recipe["recipe"])
         assert S <= MAXS
         import json
-        recipe_json[recipe_name] = json.dumps(env._recipe)
+        self.recipe_json[recipe_name] = json.dumps(env._recipe)
         env._preassembled = []
         env._success_num_conn = S
         env._max_episode_steps = 150
@@ -114,9 +137,6 @@ def main():
         for leg, table in env._recipe["recipe"]:
             for nm in (leg, table):
                 env._object_name2id.setdefault(nm, len(env._object_name2id))
-        if coef_names is None:
-            coef_names = sorted(k for k, v in vars(cfg).items() if isinstance(v, (int, float, bool)) and ("coef" in k or "threshold" in k or k in (
-                "phase_bonus", "alignment_pos_dist", "alignment_rot_dist_up", "alignment_rot_dist_forward", "alignment_project_dist")))
         w = World(rng, S)
         names = {}
         for s in range(S):
@@ -155,7 +175,7 @@ def main():
 
         def snapshot(is_reset, ac, out):
             pad = lambda a, shape: np.concatenate([a, np.zeros((MAXS - S,) + shape)]) if S < MAXS else a
-            rec["episode"].append(n_ep)
+            rec["episode"].append(self.n_ep)
             rec["is_reset"].append(is_reset)
             rec["leg_pos"].append(pad(w.leg_pos.copy(), (3,)))
             rec["leg_site_pos"].append(pad(np.stack([w.leg_site_pos(s) for s in range(S)]), (3,)))
@@ -175,8 +195,9 @@ def main():
 
         env._reset_reward_variables()
         snapshot(True, np.zeros(9), dict(reward=0.0, done=False, success=False, phase=env._phase_i, subtask=env._subtask_step, info=np.zeros(len(INFO_KEYS))))
-        for k in eps:
-            eps[k].append(S if k == "nsub" else (RECIPES.index(recipe_name) if k == "recipe" else getattr(cfg, k)))
+        if record:
+            for k in self.eps:
+                self.eps[k].append(S if k == "nsub" else (RECIPES.index(recipe_name) if k == "recipe" else getattr(cfg, k)))
         sloppy = rng.choice([0.0, 0.002, 0.01, 0.04])
         speed = rng.choice([0.35, 0.6, 1.0])
         accident = rng.choice([0.0, 0.01, 0.04])
@@ -253,26 +274,45 @@ def main():
                 w.eef = grasp + [0, 0, -0.02]
             reward, done, info = Dense._compute_reward(env, ac)
             env._episode_length += 1
-            key = (ph, bool(done), bool(env._success), int(env._subtask_step - s), int(env._phase_i))
-            branch[key] = branch.get(key, 0) + 1
+            if record:
+                key = (ph, bool(done), bool(env._success), int(env._subtask_step - s), int(env._phase_i))
+                self.branch[key] = self.branch.get(key, 0) + 1
             snapshot(False, ac, dict(reward=float(reward), done=bool(done), success=bool(env._success), phase=int(env._phase_i), subtask=int(env._subtask_step),
                                      info=np.array([float(info.get(k, 0.0)) for k in INFO_KEYS])))
             if done:
                 break
             if env._subtask_step != s:
                 table0 = w.table_pos.copy()
-        n_ep += 1
+        if record:
+            self.n_ep += 1
+        return rec["phase"]
+
+    def arrays(self):
+        """the records and the per-episode flags as the fixture stores them"""
+        return dict({k: np.array(v) for k, v in self.rec.items()}, **{"ep_" + k: np.array(v) for k, v in self.eps.items()}, recipes=np.array(RECIPES),
+                    recipe_json=np.array([self.recipe_json[r] for r in RECIPES]), info_keys=np.array(INFO_KEYS))
+
+    def report(self, name):
+        ph = np.array(self.rec["phase"])
+        print("%s: %d records, %d episodes; final phases seen %s; successes %d; subtask max %d" % (
+            name, len(ph), self.n_ep, np.bincount(ph, minlength=8).tolist(), int(np.sum(self.rec["success"])), int(np.max(self.rec["subtask"]))))
+        print("branches (phase before, done, success, subtask advance, phase after):", len(self.branch))
+        for k in sorted(self.branch):
+            print("  ", k, self.branch[k])
+
+
+def main():
+    r = Recorder()
+    rng = np.random.RandomState(20260924)
+    while len(r.rec["reward"]) < 9000:
+        r.episode(rng, r.new_config(rng))
     os.makedirs(OUT, exist_ok=True)
-    coefs = np.array([float(getattr(base_cfg, k)) for k in coef_names])
-    np.savez_compressed(os.path.join(OUT, "dense_reward.npz"), **{k: np.array(v) for k, v in rec.items()}, **{"ep_" + k: np.array(v) for k, v in eps.items()},
-                        coef_names=np.array(coef_names), coefs=coefs, recipes=np.array(RECIPES), recipe_json=np.array([recipe_json[r] for r in RECIPES]), info_keys=np.array(INFO_KEYS),
+    a = r.arrays()
+    coefs = np.array([float(getattr(r.base_cfg, k)) for k in r.coef_names])
+    np.savez_compressed(os.path.join(OUT, "dense_reward.npz"), **{k: a[k] for k in r.rec}, **{"ep_" + k: a["ep_" + k] for k in r.eps},
+                        coef_names=np.array(r.coef_names), coefs=coefs, recipes=a["recipes"], recipe_json=a["recipe_json"], info_keys=a["info_keys"],
                         source="reference furniture/env/furniture_sawyer_dense.py _compute_reward run unmodified on a scripted world (tools/make_golden_dense.py)")
-    ph = np.array(rec["phase"])
-    print("dense_reward: %d records, %d episodes; final phases seen %s; successes %d; subtask max %d" % (
-        len(ph), n_ep, np.bincount(ph, minlength=8).tolist(), int(np.sum(rec["success"])), int(np.max(rec["subtask"]))))
-    print("branches (phase before, done, success, subtask advance, phase after):", len(branch))
-    for k in sorted(branch):
-        print("  ", k, branch[k])
+    r.report("dense_reward")
 
 
 if __name__ == "__main__":
