@@ -52,8 +52,10 @@ struct FeEnvState {
   // the last observation row and qpos / qvel of the episode an env's step ended, written by that step before its auto-reset; the rows of
   // envs whose step did not end an episode are left as they are
   float *terminal_obs, *terminal_qpos, *terminal_qvel; // [N][obs_dim], [N][nq], [N][nv]
-  float* packed;                               // optional second output of a step: rows [obs | reward | done] (float), stride obs_dim + 2 --
-                                               // the send buffer of the multi-GPU all-gather, written by the step kernel itself
+  float* packed;                               // optional second output of a step: rows [obs | reward | done | info | dense_info | terminal_obs]
+                                               // (float) -- the send buffer of the multi-GPU all-gather, written by the step kernel itself
+  int pk_stride;                               // floats per packed row: obs_dim + 2 and the optional columns fe_set_packed_layout asks for
+  int pk_info, pk_dense, pk_term;              // first column of info (int32 bits), dense_info, terminal_obs in a packed row; -1 = absent
   int *group, *site_connected;                 // [N][npart], [N][nsite]
   int *num_connected, *prev_num_connected, *touched, *picked, *episode_len, *done;
   int *preassembled, *num_connects;            // [N] set_subtask (furniture.py:204-207): recipe steps connected by the env's next reset; connections asked for, -1 = None
@@ -602,18 +604,19 @@ FE_FN void fe_write_obs(FeEnv* e, float* ob, float* packed) {
   LANES_END
   }
 }
-// the env's rows of the step's outputs: obs, and the packed [obs | reward | done] row of fe_env_step_packed when it runs
+// the env's rows of the step's outputs: obs, and the obs columns of the packed row of fe_env_step_packed when it runs
 FE_HD void fe_write_step_obs(FeEnv* e) {
   const int od = e->sc->obs_dim;
-  fe_write_obs(e, e->es.obs + (size_t)e->env * od, e->es.packed ? e->es.packed + (size_t)e->env * (od + 2) : nullptr);
+  fe_write_obs(e, e->es.obs + (size_t)e->env * od, e->es.packed ? e->es.packed + (size_t)e->env * e->es.pk_stride : nullptr);
 }
 // the episode that ends in this step, before the auto-reset overwrites the slice: its last observation row (the row fe_write_step_obs would
-// have written) into terminal_obs, its qpos / qvel into terminal_qpos / terminal_qvel
+// have written) into terminal_obs and the packed row's terminal slot when the layout has one, its qpos / qvel into terminal_qpos / terminal_qvel
 FE_FN void fe_write_terminal(FeEnv* e) {
   FeWarp* w = e->w;
   const fe_model* m = w->m;
   const size_t env = (size_t)e->env;
-  fe_write_obs(e, e->es.terminal_obs + env * e->sc->obs_dim, nullptr);
+  float* pk = e->es.packed && e->es.pk_term >= 0 ? e->es.packed + env * e->es.pk_stride + e->es.pk_term : nullptr;
+  fe_write_obs(e, e->es.terminal_obs + env * e->sc->obs_dim, pk);
   float* q = e->es.terminal_qpos + env * m->nq;
   float* v = e->es.terminal_qvel + env * m->nv;
   LANES_BEGIN
@@ -967,6 +970,7 @@ FE_HD void fe_env_finish(FeEnv* e, const float* a, int act_dim, float connect, i
   // reward (furniture.py:482-541), termination (:440-445, :451-480)
   LANES_BEGIN
     if (lane == 0) {
+      float* pk = e->es.packed ? e->es.packed + (size_t)env * e->es.pk_stride : nullptr; // the env's packed row of fe_env_step_packed
       const float* coef = e->es.reward_coef + (size_t)env * 5; // success, touch, pick, ctrl_penalty, unstable_penalty
       float touch_r = 0.f, pick_r = 0.f;
       int* touched = e->es.touched + (size_t)env * np;
@@ -1006,7 +1010,8 @@ FE_HD void fe_env_finish(FeEnv* e, const float* a, int act_dim, float connect, i
         success = ds->success;
         done = done || dd;
         float* dinf = e->es.dinfo + (size_t)env * FE_DENSE_INFO;
-        for (int k = 0; k < FE_DENSE_INFO; ++k) dinf[k] = (float)di[k];
+        float* pkd = pk && e->es.pk_dense >= 0 ? pk + e->es.pk_dense : nullptr;
+        for (int k = 0; k < FE_DENSE_INFO; ++k) { dinf[k] = (float)di[k]; if (pkd) pkd[k] = (float)di[k]; }
       }
       const int len = ++e->es.episode_len[env];
       float penalty = 0.f;
@@ -1014,9 +1019,14 @@ FE_HD void fe_env_finish(FeEnv* e, const float* a, int act_dim, float connect, i
       reward += penalty;
       reward_out[env] = reward;
       done_out[env] = (uint8_t)done;
-      if (e->es.packed) { float* pk = e->es.packed + (size_t)env * (sc->obs_dim + 2) + sc->obs_dim; pk[0] = reward; pk[1] = done ? 1.f : 0.f; }
+      const int32_t iv[FE_INFO_DIM] = {nc, success, fail, len, w->u()[FE_U_NCON], w->u()[FE_U_NITER]};
+      if (pk) {
+        pk[sc->obs_dim] = reward; pk[sc->obs_dim + 1] = done ? 1.f : 0.f;
+        // the info row as int32 bit patterns, which the float32 all-gather carries unchanged
+        if (e->es.pk_info >= 0) for (int k = 0; k < FE_INFO_DIM; ++k) ((int32_t*)(pk + e->es.pk_info))[k] = iv[k];
+      }
       int32_t* info = info_out + (size_t)env * FE_INFO_DIM;
-      info[0] = nc; info[1] = success; info[2] = fail; info[3] = len; info[4] = w->u()[FE_U_NCON]; info[5] = w->u()[FE_U_NITER];
+      for (int k = 0; k < FE_INFO_DIM; ++k) info[k] = iv[k];
       e->es.done[env] = done;
       // An unstable episode resets twice, as the reference does: once inside _do_simulation's except branch
       // (furniture.py:2889-2897) and once more by the VecEnv worker because the step returned done (subproc_vec_env.py:16-20).

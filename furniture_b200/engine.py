@@ -252,6 +252,24 @@ def obs_columns(scene, robot_skip=0, robot_ob=True, object_ob=True, object_ob_al
     return cols
 
 
+def packed_columns(obs_dim, info=False, dense_info=False, terminal_obs=False):
+    """Where each block of a packed row of fe_env_step_packed sits (include/furniture_b200.h): an OrderedDict name -> slice of the row, in
+    its order obs, reward, done, then info (INFO_DIM int32 bit patterns), dense_info (DENSE_INFO_DIM floats) and terminal_obs (obs_dim
+    floats) where the layout has them.  The end of the last slice is the row's stride.  The step kernel fills the blocks of a handle's
+    layout; ShardedFurnitureEnv fills the same blocks on the host for a shard without that kernel."""
+    from collections import OrderedDict
+
+    from .dense import INFO_KEYS as DENSE_INFO_KEYS
+
+    blocks = [("obs", obs_dim, True), ("reward", 1, True), ("done", 1, True), ("info", INFO_DIM, info),
+              ("dense_info", len(DENSE_INFO_KEYS), dense_info), ("terminal_obs", obs_dim, terminal_obs)]
+    cols, o = OrderedDict(), 0
+    for name, w, present in blocks:
+        if present:
+            cols[name], o = slice(o, o + w), o + w
+    return cols
+
+
 class Engine:
     def __init__(self, model: mjcf.Model, n_envs: int, device: int = 0, config: FeConfig | None = None, lib_path: str | None = None,
                  dense: FeDenseConfig | None = None, ik=None, controller=None, obs_layout=None, fix_init=False, fix_init_parts=None,
@@ -304,6 +322,7 @@ class Engine:
             self._chk(L.fe_enable_controller(self.h, C.byref(controller)))
             self.act_dim = int(L.fe_action_dim(self.h))
         self.obs_flags = dict(OBS_DEFAULTS)
+        self.packed_flags = dict(info=False, dense_info=False, terminal_obs=False)  # set_packed_layout
         if obs_layout is not None and {**OBS_DEFAULTS, **obs_layout} != OBS_DEFAULTS:  # `obs_layout`: overrides of OBS_DEFAULTS
             self.set_obs_layout(**obs_layout)
         self._bank, self._n_pick = [], 0  # host copy of the bank of recorded starts; its first _n_pick entries are the load_init_states list
@@ -492,6 +511,21 @@ class Engine:
     def env_step_packed(self, actions_dev, packed_dev, info_dev=None, stream=None):
         """fe_env_step_packed: the kernel writes rows [obs | reward | done] straight into `packed_dev` (the all-gather send buffer)"""
         self._chk(self.L.fe_env_step_packed(self.h, C.c_void_p(actions_dev), C.c_void_p(packed_dev), C.c_void_p(info_dev or 0), C.c_void_p(stream or 0)))
+
+    def set_packed_layout(self, info=False, dense_info=False, terminal_obs=False):
+        """fe_set_packed_layout: what env_step_packed writes after [obs | reward | done] in each row, from the next packed step on: the info
+        row (int32 bit patterns), the dense reward's dense_info row (a dense handle only) and the terminal observation (valid where done)"""
+        flags = dict(info=info, dense_info=dense_info, terminal_obs=terminal_obs)
+        self._chk(self.L.fe_set_packed_layout(self.h, *[int(v) if isinstance(v, (bool, np.bool_)) else v for v in flags.values()]))
+        self.packed_flags = {k: bool(v) for k, v in flags.items()}
+
+    def packed_dim(self):
+        """fe_packed_dim: floats per packed row under the current layout and obs_dim"""
+        return int(self.L.fe_packed_dim(self.h))
+
+    def packed_columns(self):
+        """name -> slice of a packed row under this handle's layout (the module's packed_columns)"""
+        return packed_columns(self.obs_dim, **self.packed_flags)
 
     def env_step_host(self, actions):
         a = np.ascontiguousarray(actions, dtype=np.float32)

@@ -7,7 +7,8 @@ Mirrors the reference's call surface for the accelerated path:
   get_env_state / set_env_state           furniture.py:1781-1803
 Observations live in one contiguous (N, obs_dim) float32 CUDA tensor written by the step kernel; the dict entries are
 views of it.  ShardedFurnitureEnv adds the multi-GPU form: env shards are independent (one process per GPU), the only
-collective is one NCCL all_gather of the packed [obs | reward | done] tensor per step (SURVEY.md 8e).
+collective is one NCCL all_gather of the packed [obs | reward | done] tensor per step (SURVEY.md 8e), optionally widened by every
+env's info, dense_info and terminal observation.
 """
 from __future__ import annotations
 
@@ -18,7 +19,7 @@ import numpy as np
 
 from . import mjcf
 from .dense import DENSE_DEFAULTS, DENSE_ENV_DEFAULTS, INFO_KEYS as DENSE_INFO_KEYS, dense_config
-from .engine import INFO_DIM, OBS_DEFAULTS, TASK_OPTIONS, Engine, default_config
+from .engine import INFO_DIM, OBS_DEFAULTS, TASK_OPTIONS, Engine, default_config, packed_columns
 
 RESET_DEFAULTS = dict(fix_init=False, fix_init_parts=None, reset_robot_after_attach=False, assembled=False)  # config/furniture.py:116-127, :169-174, :307-312
 SIM_DEFAULTS = dict(control_freq=10, no_collision=False)  # config/furniture.py:71-73, :304-306
@@ -468,6 +469,7 @@ class MixedFurnitureEnv:
         self._act = torch.empty((off, self.act_dim), dtype=torch.float32, device=self.device)
         self._streams = [torch.cuda.Stream(device=self.device) for _ in self.buckets]
         self._term_obs = torch.zeros_like(self._obs)  # terminal_observation's rows, laid out like _obs
+        self.dense_cfg = b0.dense_cfg  # every bucket is built with the same reward
         self._term_views, o = OrderedDict(), 0
         for k, w in widths.items():
             self._term_views[k], o = self._term_obs[:, o : o + w], o + w
@@ -562,6 +564,16 @@ class MixedFurnitureEnv:
                 self._term_views[k][off : off + b.num_envs, : v.shape[1]].copy_(v)
         return self._obs_dict(self._term_obs)
 
+    def dense_infos(self):
+        """(num_envs, 12) float32 tensor of every bucket's dense_info rows after the last step, in global env order and the order of
+        dense.INFO_KEYS; padding rows are zeros (a host round trip per bucket)"""
+        if self.dense_cfg is None:
+            raise RuntimeError("this env runs the sparse reward")
+        rows = self.torch.zeros((self.num_envs, len(DENSE_INFO_KEYS)), dtype=self.torch.float32, device=self.device)
+        for b, off in zip(self.buckets, self.offsets):
+            rows[off : off + b.num_envs] = self.torch.from_numpy(b.engine.get("dense_info"))
+        return rows
+
     def terminal_state(self):
         """BatchedFurnitureEnv.terminal_state of every bucket, in bucket order (bucket i holds the envs from offsets[i] on): the models' nq and nv
         differ, so the states are not stacked"""
@@ -625,9 +637,16 @@ def shard_furniture(names, envs_per_model, world, nv=None, envs_per_rank=None, c
 
 class ShardedFurnitureEnv:
     """One process per GPU (torch.distributed, backend nccl). Each rank steps its own contiguous env shard; after the
-    step one all_gather makes the packed [obs | reward | done] of every shard visible on every rank."""
+    step one all_gather makes the packed [obs | reward | done] of every shard visible on every rank.
 
-    def __init__(self, envs_per_gpu, agent="Sawyer", furniture_name="table_lack_0825", env=None, **cfg_overrides):
+    `gather_info` widens the message by each env's info row (and, on a dense-reward shard, its dense_info row), so that step returns the
+    info of every env and dense_infos() the dense rows of every env; `gather_terminal` widens it by the terminal observation, which
+    terminal_observation() returns for every env.  The step kernel writes the wider rows itself (Engine.set_packed_layout); a shard
+    without that kernel (MixedFurnitureEnv, a stand-in) has the same columns filled from its own step, terminal_observation() and
+    dense_infos()."""
+
+    def __init__(self, envs_per_gpu, agent="Sawyer", furniture_name="table_lack_0825", env=None, gather_info=False, gather_terminal=False,
+                 **cfg_overrides):
         import torch
         import torch.distributed as dist
 
@@ -639,7 +658,14 @@ class ShardedFurnitureEnv:
         self.env = env if env is not None else BatchedFurnitureEnv(agent, furniture_name, envs_per_gpu, device=local, **cfg_overrides)
         self.envs_per_gpu = envs_per_gpu
         self.num_envs = envs_per_gpu * self.world
-        self.pack_dim = self.env.obs_dim + 2
+        self.gather_info, self.gather_terminal = bool(gather_info), bool(gather_terminal)
+        layout = dict(info=self.gather_info, dense_info=self.gather_info and getattr(self.env, "dense_cfg", None) is not None,
+                      terminal_obs=self.gather_terminal)
+        self._cols = packed_columns(self.env.obs_dim, **layout)
+        self._kernel = hasattr(self.env, "_stream")  # a BatchedFurnitureEnv: its step kernel writes the rows
+        if self._kernel:
+            self.env.engine.set_packed_layout(**layout)
+        self.pack_dim = next(reversed(self._cols.values())).stop
         self._pack = torch.empty((envs_per_gpu, self.pack_dim), dtype=torch.float32, device=self.env.device)
         self._all = torch.empty((self.num_envs, self.pack_dim), dtype=torch.float32, device=self.env.device)
         self.timing, self._events = False, []
@@ -657,14 +683,31 @@ class ShardedFurnitureEnv:
         self.env.reset()
         p = self._pack  # resets are rare: packed on the host side of the stream (the step kernel writes its own rows)
         p[:, : self.env.obs_dim] = self.env._obs
-        p[:, self.env.obs_dim :] = 0
+        p[:, self.env.obs_dim :] = 0  # reward, done and the info, dense_info and terminal columns
         allp = self._gather()
         return self.env._obs_dict(allp[:, : self.env.obs_dim])
 
+    def _pack_on_host(self, a):
+        """the rows of a shard without the packed step kernel, filled from its own outputs into the same columns"""
+        env, c, p = self.env, self._cols, self._pack
+        od_, rew, done, info = env.step(a)
+        p[:, c["obs"]] = env._obs
+        p[:, c["reward"]] = rew.reshape(-1, 1)
+        p[:, c["done"]] = done.float().reshape(-1, 1)
+        if "info" in c:
+            p[:, c["info"]].view(self.torch.int32).copy_(info)  # bit patterns, as the kernel writes them
+        if "dense_info" in c:
+            p[:, c["dense_info"]] = env.dense_infos()
+        if "terminal_obs" in c:
+            p[:, c["terminal_obs"]] = self.torch.cat(list(env.terminal_observation().values()), 1)
+        return info
+
     def step(self, local_actions):
         """One env step of the local shard, then the single collective of the data path.  The step kernel writes
-        [obs | reward | done] rows into the registered send buffer itself (fe_env_step_packed); with `timing` set, CUDA events
-        separate the kernel from the time spent in the all-gather (which includes waiting for the slowest rank)."""
+        the packed rows into the registered send buffer itself (fe_env_step_packed); with `timing` set, CUDA events
+        separate the kernel from the time spent in the all-gather (which includes waiting for the slowest rank).
+        Returns the gathered obs dict, rewards and dones, and the info of every env under gather_info (an int32 view of the message),
+        else this shard's own info."""
         env, t = self.env, self.torch
         a = t.as_tensor(local_actions["default"] if isinstance(local_actions, dict) else local_actions)
         if a.device != env.device or a.dtype != t.float32 or not a.is_contiguous():
@@ -674,22 +717,35 @@ class ShardedFurnitureEnv:
         if self.timing:
             ev = [t.cuda.Event(enable_timing=True) for _ in range(3)]
             ev[0].record()
-        if hasattr(env, "_stream"):
+        if self._kernel:
             env.engine.env_step_packed(a.data_ptr(), self._pack.data_ptr(), env._info.data_ptr(), stream=env._stream())
             info = env._info
-        else:  # stand-in shard of the gloo tests
-            od_, rew, done, info = env.step(a)
-            self._pack[:, : env.obs_dim] = env._obs
-            self._pack[:, env.obs_dim] = rew
-            self._pack[:, env.obs_dim + 1] = done.float()
+        else:  # MixedFurnitureEnv, or the stand-in shard of the gloo tests
+            info = self._pack_on_host(a)
         if self.timing:
             ev[1].record()
         allp = self._gather()
         if self.timing:
             ev[2].record()
             self._events.append(ev)
-        od = env.obs_dim
-        return env._obs_dict(allp[:, :od]), allp[:, od], allp[:, od + 1] > 0.5, info
+        c = self._cols
+        if "info" in c:
+            info = allp[:, c["info"]].view(t.int32)
+        return env._obs_dict(allp[:, c["obs"]]), allp[:, c["reward"].start], allp[:, c["done"].start] > 0.5, info
+
+    def terminal_observation(self):
+        """the terminal observation of every env (gather_terminal=True): an obs dict with step()'s keys, views of the last gathered message;
+        row i is valid where the last gathered done[i] is 1"""
+        if "terminal_obs" not in self._cols:
+            raise ValueError("terminal_observation() needs ShardedFurnitureEnv(..., gather_terminal=True)")
+        return self.env._obs_dict(self._all[:, self._cols["terminal_obs"]])
+
+    def dense_infos(self):
+        """(num_envs, 12) float32 rows of the dense reward's dense_info of every env after the last gathered step (gather_info=True on a
+        dense-reward shard), in the order of dense.INFO_KEYS; views of the message"""
+        if "dense_info" not in self._cols:
+            raise ValueError("dense_infos() needs ShardedFurnitureEnv(..., gather_info=True) on a shard that runs the dense reward")
+        return self._all[:, self._cols["dense_info"]]
 
     def local_slice(self, gathered):
         """rows of this rank's own shard in a gathered (num_envs, ...) tensor"""

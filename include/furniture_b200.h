@@ -207,10 +207,23 @@ int fe_set_init_states(fe_handle* h, const float* qpos_host, const float* qvel_h
 int fe_env_reset(fe_handle* h, const uint8_t* env_mask_dev /* NULL = all */, float* obs_dev, void* stream);
 int fe_env_step(fe_handle* h, const float* actions_dev, float* obs_dev, float* reward_dev, uint8_t* done_dev, int32_t* info_dev,
                 void* stream);
-/* same step, results written by the kernel as rows [obs | reward | done] of (obs_dim + 2) floats: the send buffer of the
-   observation all-gather over env shards (SURVEY.md 8e; the reference's counterpart is the pipe of
-   util/subproc_vec_env.py:100-113 that carries (ob, reward, done, info) of every worker back to the caller) */
+/* same step, results written by the kernel as rows of fe_packed_dim(h) floats: the send buffer of the observation all-gather over env
+   shards (SURVEY.md 8e; the reference's counterpart is the pipe of util/subproc_vec_env.py:100-113 that carries (ob, reward, done, info)
+   of every worker back to the caller).  A row is, in this order:
+     obs           obs_dim floats, the row fe_env_step writes to obs
+     reward, done  2 floats (done 0 or 1)
+     info          FE_INFO_DIM = 6 floats holding the int32 bit patterns of the env's info row, so that they survive a float32 all-gather
+                   exactly (read them through an int32 view)                                 -- with fe_set_packed_layout's info = 1
+     dense_info    fe_dense_info_dim() floats, the step's row of field "dense_info"          -- with dense_info = 1
+     terminal_obs  obs_dim floats, the row the step also writes to terminal_obs              -- with terminal_obs = 1
+   The terminal slot of a row is valid where that step's done is 1 and is left untouched otherwise, exactly like terminal_obs.  With the
+   default layout the rows are [obs | reward | done], obs_dim + 2 floats, and nothing past them is written. */
 int fe_env_step_packed(fe_handle* h, const float* actions_dev, float* packed_dev, int32_t* info_dev, void* stream);
+/* What fe_env_step_packed writes after [obs | reward | done]: each flag 0 or 1, in effect from the next packed step.  Refused for a flag
+   outside {0, 1}, for dense_info on a handle without the dense reward, and for a handle created without a scene blob. */
+int fe_set_packed_layout(fe_handle* h, int info, int dense_info, int terminal_obs);
+/* floats per packed row under the handle's layout at its current obs_dim (it follows fe_set_obs_layout): obs_dim + 2 by default */
+int fe_packed_dim(const fe_handle* h);
 /* same call with host buffers: H2D of the actions and D2H of the results happen inside (pinned staging) */
 int fe_env_step_host(fe_handle* h, const float* actions_host, float* obs_host, float* reward_host, uint8_t* done_host, int32_t* info_host);
 /* FurnitureGym.set_max_episode_steps -> FurnitureEnv.set_max_episode_steps (furniture_gym.py:35-37, furniture.py:271-272):
@@ -229,7 +242,7 @@ int fe_enable_dense_reward(fe_handle* h, const fe_dense_config* dc);
  * of every reset; with the dense reward, the recipe step's (leg, table) from each reset and from each move to the next subtask on, which the
  * observation shows from the following step (the observation of a step is taken before its reward, furniture_sawyer.py:66-84).  Field
  * "subtask_part" holds the pair.  Call before the first fe_env_reset or env step; it is refused after, and for a flag outside {0, 1}.
- * fe_obs_dim reports the new width, the obs buffer is reallocated (fe_obs_dev moves), and packed rows keep the stride obs_dim + 2. */
+ * fe_obs_dim reports the new width, the obs buffer is reallocated (fe_obs_dev moves), and packed rows take the new width (fe_packed_dim). */
 int fe_set_obs_layout(fe_handle* h, int robot_ob, int object_ob, int object_ob_all, int subtask_ob);
 int fe_dense_info_dim(void);
 /* device pointer of the internal obs buffer after the last step/reset: (n_envs, obs_dim) float32 */

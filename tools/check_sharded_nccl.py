@@ -1,7 +1,8 @@
 """Multi-GPU check of ShardedFurnitureEnv over NCCL (run under torchrun, one rank per GPU):
   torchrun --nnodes=1 --nproc-per-node 2 --master-addr 127.0.0.1 --master-port 29511 tools/check_sharded_nccl.py
 Every rank steps its own shard; the all-gathered [obs | reward | done] must contain every rank's local tensors bit for
-bit, the shards must differ (per-rank seeds), and a shard must be bit-identical to the same envs stepped alone."""
+bit, the shards must differ (per-rank seeds), and a shard must be bit-identical to the same envs stepped alone.  The full message
+(gather_info, gather_terminal; episodes of 2 steps) must carry every rank's info and, where done, terminal observation bit for bit."""
 import os
 import sys
 
@@ -42,6 +43,25 @@ for k in range(3):
     other = full[((rank + 1) % world) * n : ((rank + 1) % world + 1) * n]
     assert not torch.allclose(other[:, :2], mine[:, :2]), "shards with different seeds placed parts identically"
     assert torch.isfinite(full).all()
+# the full message: [obs | reward | done | info | terminal_obs]
+full = ShardedFurnitureEnv(n, gather_info=True, gather_terminal=True, max_episode_steps=2)
+alone = BatchedFurnitureEnv("Sawyer", "table_lack_0825", n, device=local, seed=ShardedFurnitureEnv.shard_seed(123, rank, n), max_episode_steps=2)
+full.reset()
+alone.reset()
+for k in range(3):
+    a = torch.rand((n, full.env.act_dim), device=dev, generator=gen) * 2 - 1
+    od, rew, done, info = full.step(a)
+    alone.step(a)
+    assert info.shape == (n * world, 6) and info.dtype == torch.int32
+    parts = [torch.zeros_like(alone._info) for _ in range(world)]
+    dist.all_gather(parts, alone._info)
+    assert torch.equal(info, torch.cat(parts, 0)), "the gathered info is not every rank's info"
+    mine = torch.cat(list(alone.terminal_observation().values()), 1).contiguous()
+    parts = [torch.zeros_like(mine) for _ in range(world)]
+    dist.all_gather(parts, mine)
+    to = torch.cat(list(full.terminal_observation().values()), 1)
+    d = done.bool()
+    assert d.any() == (k == 1) and torch.equal(to[d], torch.cat(parts, 0)[d]), "the gathered terminal rows are not every rank's"
 km, gm = env.pop_timing()
 assert len(km) == 3 and all(v > 0 for v in km + gm)
 dist.barrier()
