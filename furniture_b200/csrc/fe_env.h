@@ -14,6 +14,8 @@
 #define FE_SCENE_MAGIC 0x46455344 /* "FESD" */
 #define FE_MAXCONN 48
 #define FE_INFO_DIM 6
+#define FE_REWARD_INFO 4  /* success_reward, touch_reward, pick_reward, ctrl_penalty of FurnitureEnv._compute_reward (furniture.py:535-540) */
+#define FE_EPISODE_INFO 2 /* episode_reward, episode_unstable of FurnitureEnv._after_step (furniture.py:469-476) */
 
 // the observation flags of config/furniture.py (robot_ob, object_ob, object_ob_all, subtask_ob; read at furniture.py:103-107) as the bits of
 // fe_scene.obs_layout, each set where the flag differs from its default, so that 0 is the default row [object_ob (7 per part) | robot_ob]
@@ -56,6 +58,7 @@ struct FeEnvState {
                                                // (float) -- the send buffer of the multi-GPU all-gather, written by the step kernel itself
   int pk_stride;                               // floats per packed row: obs_dim + 2 and the optional columns fe_set_packed_layout asks for
   int pk_info, pk_dense, pk_term;              // first column of info (int32 bits), dense_info, terminal_obs in a packed row; -1 = absent
+  int pk_step;                                 // first column of the step-info block [reward_info | episode_info] (fe_set_packed_step_info); -1 = absent
   int *group, *site_connected;                 // [N][npart], [N][nsite]
   int *num_connected, *prev_num_connected, *touched, *picked, *episode_len, *done;
   int *preassembled, *num_connects;            // [N] set_subtask (furniture.py:204-207): recipe steps connected by the env's next reset; connections asked for, -1 = None
@@ -85,7 +88,11 @@ struct FeEnvState {
   float* reward_coef;                          // [N][5] success_reward, touch_reward, pick_reward, ctrl_penalty_coef, unstable_penalty_coef (:291-295)
   int* max_episode_steps;                      // [N] (:163-168)
   int *robot_contype, *robot_conaff;           // [N][ngeom] saved robot masks during reset
-  float* episode_reward;
+  float* episode_reward;                       // [N] _episode_reward: the rewards of the episode so far, before the unstable penalty (furniture.py:459-461)
+  // the step's info dict (furniture.py:451-541): the sparse reward's four terms of every step (NULL on a dense handle, whose terms are dinfo),
+  // and {episode_reward + penalty, episode_unstable = penalty} of the episode a step ended, written by that step; other rows are left as they are
+  float* reward_info;                          // [N][FE_REWARD_INFO] success_reward, touch_reward, pick_reward, ctrl_penalty
+  float* episode_info;                         // [N][FE_EPISODE_INFO]
   // dense (phase-based) reward, fe_dense.h: NULL = the sparse reward of FurnitureEnv._compute_reward
   const fe_dense_config* dense;                // [N] each env's coefficients and flags; lane 0 reads its row once per step
   FeDenseState* dstate;                        // [N]
@@ -991,6 +998,10 @@ FE_HD void fe_env_finish(FeEnv* e, const float* a, int act_dim, float connect, i
       float sq = 0.f;
       for (int k = 0; k < act_dim; ++k) sq += a[k] * a[k];
       float reward = success_r + touch_r + pick_r - coef[3] * sq;
+      // _compute_reward's info (furniture.py:535-540): the terms the reward is made of.  ctrl_penalty (_ctrl_penalty, :549) is the part of the
+      // reward the control penalty makes: the reward less the other three in their order.  That is -coef[3] * sq, up to the single rounding
+      // of the product the device fuses into the reward, and the four terms add up to the reward exactly.
+      const float terms[FE_REWARD_INFO] = {success_r, touch_r, pick_r, reward - (success_r + touch_r + pick_r)};
       const int n_goal = e->es.success_num_conn[env];
       int success = (nc == n_goal && np > 1) ? 1 : 0;
       int done = success;
@@ -1014,16 +1025,28 @@ FE_HD void fe_env_finish(FeEnv* e, const float* a, int act_dim, float connect, i
         for (int k = 0; k < FE_DENSE_INFO; ++k) { dinf[k] = (float)di[k]; if (pkd) pkd[k] = (float)di[k]; }
       }
       const int len = ++e->es.episode_len[env];
+      // _after_step (furniture.py:459-476): the episode's return before the penalty.  After an unstable step the reset inside the step has
+      // zeroed it, as _do_simulation's except branch does (:2889-2897 -> _after_reset :355-356), so that episode reports this step alone.
+      const float ep_r = e->es.episode_reward[env] += reward;
       float penalty = 0.f;
       if (len == e->es.max_episode_steps[env] || fail) { done = 1; if (fail) penalty = -coef[4]; }
       reward += penalty;
       reward_out[env] = reward;
       done_out[env] = (uint8_t)done;
       const int32_t iv[FE_INFO_DIM] = {nc, success, fail, len, w->u()[FE_U_NCON], w->u()[FE_U_NITER]};
+      const float ep[FE_EPISODE_INFO] = {ep_r + penalty, penalty};
+      if (e->es.reward_info) for (int k = 0; k < FE_REWARD_INFO; ++k) e->es.reward_info[(size_t)env * FE_REWARD_INFO + k] = terms[k];
+      if (done) for (int k = 0; k < FE_EPISODE_INFO; ++k) e->es.episode_info[(size_t)env * FE_EPISODE_INFO + k] = ep[k];
       if (pk) {
         pk[sc->obs_dim] = reward; pk[sc->obs_dim + 1] = done ? 1.f : 0.f;
         // the info row as int32 bit patterns, which the float32 all-gather carries unchanged
         if (e->es.pk_info >= 0) for (int k = 0; k < FE_INFO_DIM; ++k) ((int32_t*)(pk + e->es.pk_info))[k] = iv[k];
+        // the step-info block: the reward terms (NaN on a dense handle, which has none), the episode record where done as in episode_info
+        if (e->es.pk_step >= 0) {
+          float* ps = pk + e->es.pk_step;
+          for (int k = 0; k < FE_REWARD_INFO; ++k) ps[k] = e->es.reward_info ? terms[k] : nanf("");
+          if (done) for (int k = 0; k < FE_EPISODE_INFO; ++k) ps[FE_REWARD_INFO + k] = ep[k];
+        }
       }
       int32_t* info = info_out + (size_t)env * FE_INFO_DIM;
       for (int k = 0; k < FE_INFO_DIM; ++k) info[k] = iv[k];

@@ -22,6 +22,10 @@ DEFAULT_LIB = os.path.join(_HERE, "libfurniture_b200.so")
 MAXCONN = 48
 SCENE_MAGIC = 0x46455344
 INFO_DIM = 6
+# the step's info dict of the reference (FurnitureEnv._compute_reward / _after_step, furniture.py:451-541): fields "reward_info" and
+# "episode_info" (include/furniture_b200.h) in this column order
+REWARD_INFO_KEYS = ("success_reward", "touch_reward", "pick_reward", "ctrl_penalty")
+EPISODE_INFO_KEYS = ("episode_reward", "episode_unstable")
 # bits of the `flags` field and columns of the `stats` field: FE_FLAG_* / FE_STAT_* of include/furniture_b200.h, which says what each means
 FLAG_CONTACT_FULL, FLAG_NUMERIC, FLAG_NEWTON_PIVOT, FLAG_DIVERGED = 1, 2, 4, 8
 STAT_PART_ITERS, STAT_COUPLED, STAT_NEWTON_SOLVES, STAT_NEWTON_ITERS = 0, 1, 2, 3
@@ -252,17 +256,19 @@ def obs_columns(scene, robot_skip=0, robot_ob=True, object_ob=True, object_ob_al
     return cols
 
 
-def packed_columns(obs_dim, info=False, dense_info=False, terminal_obs=False):
+def packed_columns(obs_dim, info=False, dense_info=False, terminal_obs=False, step_info=False):
     """Where each block of a packed row of fe_env_step_packed sits (include/furniture_b200.h): an OrderedDict name -> slice of the row, in
-    its order obs, reward, done, then info (INFO_DIM int32 bit patterns), dense_info (DENSE_INFO_DIM floats) and terminal_obs (obs_dim
-    floats) where the layout has them.  The end of the last slice is the row's stride.  The step kernel fills the blocks of a handle's
+    its order obs, reward, done, then info (INFO_DIM int32 bit patterns), dense_info (DENSE_INFO_DIM floats), terminal_obs (obs_dim
+    floats), reward_info (the 4 REWARD_INFO_KEYS, NaN on a dense handle) and episode_info (the 2 EPISODE_INFO_KEYS, valid where done) where
+    the layout has them; step_info gives the last two together.  The end of the last slice is the row's stride.  The step kernel fills the blocks of a handle's
     layout; ShardedFurnitureEnv fills the same blocks on the host for a shard without that kernel."""
     from collections import OrderedDict
 
     from .dense import INFO_KEYS as DENSE_INFO_KEYS
 
     blocks = [("obs", obs_dim, True), ("reward", 1, True), ("done", 1, True), ("info", INFO_DIM, info),
-              ("dense_info", len(DENSE_INFO_KEYS), dense_info), ("terminal_obs", obs_dim, terminal_obs)]
+              ("dense_info", len(DENSE_INFO_KEYS), dense_info), ("terminal_obs", obs_dim, terminal_obs),
+              ("reward_info", len(REWARD_INFO_KEYS), step_info), ("episode_info", len(EPISODE_INFO_KEYS), step_info)]
     cols, o = OrderedDict(), 0
     for name, w, present in blocks:
         if present:
@@ -289,7 +295,7 @@ class Engine:
         L.fe_field_dtype.argtypes = [C.c_void_p, C.c_char_p]
         for f in ("fe_model_sizeof", "fe_scene_sizeof", "fe_config_sizeof"):
             getattr(L, f).restype = C.c_size_t
-        for f in ("fe_obs_dev", "fe_terminal_obs_dev", "fe_terminal_qpos_dev", "fe_terminal_qvel_dev"):
+        for f in ("fe_obs_dev", "fe_terminal_obs_dev", "fe_terminal_qpos_dev", "fe_terminal_qvel_dev", "fe_reward_info_dev", "fe_episode_info_dev"):
             getattr(L, f).restype = C.c_void_p
             getattr(L, f).argtypes = [C.c_void_p]
         self.is_cuda = bool(L.fe_is_cuda())
@@ -322,7 +328,7 @@ class Engine:
             self._chk(L.fe_enable_controller(self.h, C.byref(controller)))
             self.act_dim = int(L.fe_action_dim(self.h))
         self.obs_flags = dict(OBS_DEFAULTS)
-        self.packed_flags = dict(info=False, dense_info=False, terminal_obs=False)  # set_packed_layout
+        self.packed_flags = dict(info=False, dense_info=False, terminal_obs=False, step_info=False)  # set_packed_layout, set_packed_step_info
         if obs_layout is not None and {**OBS_DEFAULTS, **obs_layout} != OBS_DEFAULTS:  # `obs_layout`: overrides of OBS_DEFAULTS
             self.set_obs_layout(**obs_layout)
         self._bank, self._n_pick = [], 0  # host copy of the bank of recorded starts; its first _n_pick entries are the load_init_states list
@@ -517,7 +523,13 @@ class Engine:
         row (int32 bit patterns), the dense reward's dense_info row (a dense handle only) and the terminal observation (valid where done)"""
         flags = dict(info=info, dense_info=dense_info, terminal_obs=terminal_obs)
         self._chk(self.L.fe_set_packed_layout(self.h, *[int(v) if isinstance(v, (bool, np.bool_)) else v for v in flags.values()]))
-        self.packed_flags = {k: bool(v) for k, v in flags.items()}
+        self.packed_flags.update((k, bool(v)) for k, v in flags.items())
+
+    def set_packed_step_info(self, step_info=True):
+        """fe_set_packed_step_info: whether env_step_packed writes the step-info block [reward_info | episode_info] after the blocks of
+        set_packed_layout, from the next packed step on"""
+        self._chk(self.L.fe_set_packed_step_info(self.h, int(step_info) if isinstance(step_info, (bool, np.bool_)) else step_info))
+        self.packed_flags["step_info"] = bool(step_info)
 
     def packed_dim(self):
         """fe_packed_dim: floats per packed row under the current layout and obs_dim"""
@@ -701,6 +713,23 @@ class Engine:
         """device pointers of the terminal buffers: (obs (N, obs_dim), qpos (N, nq), qvel (N, nv)), float32, env-major; the obs pointer moves
         with set_obs_layout"""
         return self.L.fe_terminal_obs_dev(self.h), self.L.fe_terminal_qpos_dev(self.h), self.L.fe_terminal_qvel_dev(self.h)
+
+    # ---- the step's info dict (furniture.py:451-541): fields "reward_info" and "episode_info", written by every env step
+    def reward_info(self):
+        """(N, 4) float32 host copy of the last step's reward terms in the order of REWARD_INFO_KEYS (a sparse-reward handle only: a dense
+        handle has no such terms: its steps write none, and this raises)"""
+        if self.dense is not None:
+            raise RuntimeError("this handle runs the dense reward: its reward terms are the field dense_info")
+        return self.get("reward_info")
+
+    def episode_info(self):
+        """(N, 2) float32 host copy of the episode record in the order of EPISODE_INFO_KEYS, valid where the last step's done is 1; rows no
+        step has written are NaN"""
+        return self.get("episode_info")
+
+    def step_info_dev_ptrs(self):
+        """device pointers of (reward_info (N, 4), episode_info (N, 2)), float32, env-major; reward_info is None on a dense handle"""
+        return self.L.fe_reward_info_dev(self.h), self.L.fe_episode_info_dev(self.h)
 
     def is_aligned(self, p1, m1, p2, m2, angles, nangles, thr):
         n = len(p1)

@@ -13,13 +13,14 @@ env's info, dense_info and terminal observation.
 from __future__ import annotations
 
 import os
+import time
 from collections import OrderedDict
 
 import numpy as np
 
 from . import mjcf
 from .dense import DENSE_DEFAULTS, DENSE_ENV_DEFAULTS, INFO_KEYS as DENSE_INFO_KEYS, dense_config
-from .engine import INFO_DIM, OBS_DEFAULTS, TASK_OPTIONS, Engine, default_config, packed_columns
+from .engine import EPISODE_INFO_KEYS, INFO_DIM, OBS_DEFAULTS, REWARD_INFO_KEYS, TASK_OPTIONS, Engine, default_config, packed_columns
 
 RESET_DEFAULTS = dict(fix_init=False, fix_init_parts=None, reset_robot_after_attach=False, assembled=False)  # config/furniture.py:116-127, :169-174, :307-312
 SIM_DEFAULTS = dict(control_freq=10, no_collision=False)  # config/furniture.py:71-73, :304-306
@@ -267,6 +268,13 @@ class BatchedFurnitureEnv:
         self._term_obs = device_view(tob, (num_envs, self.obs_dim), self.device)
         self._term_qpos = device_view(tq, (num_envs, self.model.nq), self.device)
         self._term_qvel = device_view(tv, (num_envs, self.model.nv), self.device)
+        # the step's info dict (furniture.py:451-541), written by the step kernel: reward terms (sparse handles only) and episode records
+        ri, ei = e.step_info_dev_ptrs()
+        self._reward_info = device_view(ri, (num_envs, len(REWARD_INFO_KEYS)), self.device) if ri else None
+        self._episode_info = device_view(ei, (num_envs, len(EPISODE_INFO_KEYS)), self.device)
+        self.narms = int(e.scene.narms)
+        self._last = None  # (done, info, actions) of the last step, tensors or host arrays, for step_infos
+        self._episode_start = np.full(num_envs, time.time())  # host clock of each env's last reset seen by reset() / step_infos()
 
     def set_init_qpos(self, states):
         """FurnitureEnv.set_init_qpos (furniture.py:315-316), per env: one get_env_state dict or None for all envs, or a list of num_envs of
@@ -357,6 +365,7 @@ class BatchedFurnitureEnv:
             mask = mask.to(device=self.device, dtype=self.torch.uint8).contiguous()
             m = mask.data_ptr()
         self.engine.env_reset(mask_dev=m, obs_dev=self._obs.data_ptr(), stream=self._stream())
+        self._episode_start[mask.bool().cpu().numpy() if mask is not None else slice(None)] = time.time()
         return self._obs_dict(self._obs)
 
     def step(self, actions):
@@ -370,11 +379,13 @@ class BatchedFurnitureEnv:
             a = self._act
         assert a.shape == (self.num_envs, self.act_dim), tuple(a.shape)
         self.engine.env_step_dev(a.data_ptr(), self._obs.data_ptr(), self._rew.data_ptr(), self._done.data_ptr(), self._info.data_ptr(), stream=self._stream())
+        self._last = (self._done, self._info, a.clone() if self.narms == 2 else None)  # FurnitureBaxterEnv's info["ac"]
         return self._obs_dict(self._obs), self._rew, self._done, self._info
 
     def step_host(self, actions_np):
         """numpy in / numpy out through fe_env_step_host (pinned staging, copies inside the call)."""
         obs, rew, done, info = self.engine.env_step_host(actions_np)
+        self._last = (done, info, np.array(actions_np, np.float32) if self.narms == 2 else None)
         return self._obs_dict(obs), rew, done.astype(bool), info
 
     def terminal_observation(self):
@@ -392,6 +403,58 @@ class BatchedFurnitureEnv:
     def infos(self):
         info = self._info.cpu().numpy()
         return tuple({k: int(row[j]) for j, k in enumerate(INFO_KEYS)} for row in info)
+
+    def reward_terms(self):
+        """_compute_reward's info of the last step (furniture.py:535-540): {success_reward, touch_reward, pick_reward, ctrl_penalty}, each an
+        (N,) float32 view of the device row the step kernel writes.  Where the step was not unstable, ((success_reward + touch_reward) +
+        pick_reward) + ctrl_penalty is the step's reward, bit for bit; an unstable step's reward adds episode_unstable.  The dense env
+        never runs that reward: its terms are dense_infos(), and this raises."""
+        if self._reward_info is None:
+            raise RuntimeError("this env runs the dense reward: its reward terms are dense_infos()")
+        return OrderedDict((k, self._reward_info[:, j]) for j, k in enumerate(REWARD_INFO_KEYS))
+
+    def episode_record(self):
+        """_after_step's episode_reward and episode_unstable (furniture.py:469-476) of the episode the last step ended: (N,) float32 views of
+        the device rows the step kernel writes before its auto-reset, valid where that step's done is 1 (the other rows are left as they
+        were; rows no step has written are NaN).  episode_reward is the float32 sum of the episode's rewards before the penalty, plus the
+        penalty; after an unstable step the episode is that step alone, as in the reference (furniture.py:2889-2897, :355-356)."""
+        return OrderedDict((k, self._episode_info[:, j]) for j, k in enumerate(EPISODE_INFO_KEYS))
+
+    def step_infos(self):
+        """the tuple of N info dicts that the reference's SubprocVecEnv.step_wait returns for the last step (subproc_vec_env.py:100-113),
+        with the keys of FurnitureEnv.step in its order (furniture.py:451-541, furniture_baxter.py:66-79): the sparse reward's four terms
+        (the dense env: its dense_info keys), "ac" on the two-arm env, and at done the six episode_* keys, with episode_success_state (the
+        terminal state, get_env_state's dict) on success.  episode_time is the host clock since the env's last reset that reset() or this
+        method saw; every other value is the step kernel's.  One host round trip."""
+        if self._last is None:
+            raise RuntimeError("step_infos() describes the last step: call step() first")
+        host = lambda x: x.cpu().numpy() if hasattr(x, "cpu") else np.asarray(x)
+        done, info, act = host(self._last[0]).astype(bool), host(self._last[1]), self._last[2]
+        terms = self.engine.get("dense_info") if self._reward_info is None else host(self._reward_info)
+        keys = DENSE_INFO_KEYS if self._reward_info is None else REWARD_INFO_KEYS
+        now = time.time()
+        ep = host(self._episode_info) if done.any() else None
+        success_state = None
+        if done.any() and info[done, 1].any():
+            success_state = {k: host(v) for k, v in self.terminal_state().items()}
+        act = host(act) if act is not None else None
+        out = []
+        for i in range(self.num_envs):
+            d = OrderedDict((k, float(terms[i, j])) for j, k in enumerate(keys))
+            if act is not None:
+                d["ac"] = act[i].copy()
+            if done[i]:
+                d["episode_success"] = int(info[i, 1])
+                d["episode_reward"] = float(ep[i, 0])
+                d["episode_length"] = int(info[i, 3])
+                d["episode_time"] = now - float(self._episode_start[i])
+                d["episode_unstable"] = float(ep[i, 1])
+                d["episode_num_connected"] = int(info[i, 0])
+                if info[i, 1]:
+                    d["episode_success_state"] = {k: v[i].astype(np.float64) for k, v in success_state.items()}
+                self._episode_start[i] = now
+            out.append(d)
+        return tuple(out)
 
     def get_env_state(self):
         q, v = self.engine.get_state()
@@ -574,6 +637,34 @@ class MixedFurnitureEnv:
             rows[off : off + b.num_envs] = self.torch.from_numpy(b.engine.get("dense_info"))
         return rows
 
+    def _gather_rows(self, rows_of, width):
+        """(num_envs, width) float32 tensor of every bucket's rows_of(bucket) in global env order; padding rows are NaN"""
+        rows = self.torch.full((self.num_envs, width), float("nan"), dtype=self.torch.float32, device=self.device)
+        for b, off in zip(self.buckets, self.offsets):
+            rows[off : off + b.num_envs] = rows_of(b)
+        return rows
+
+    def reward_terms(self):
+        """BatchedFurnitureEnv.reward_terms of every bucket in global env order: {success_reward, touch_reward, pick_reward, ctrl_penalty},
+        each a (num_envs,) float32 tensor (padding rows NaN)"""
+        if self.dense_cfg is not None:
+            raise RuntimeError("this env runs the dense reward: its reward terms are dense_infos()")
+        rows = self._gather_rows(lambda b: b._reward_info, len(REWARD_INFO_KEYS))
+        return OrderedDict((k, rows[:, j]) for j, k in enumerate(REWARD_INFO_KEYS))
+
+    def episode_record(self):
+        """BatchedFurnitureEnv.episode_record of every bucket in global env order: {episode_reward, episode_unstable}, each a (num_envs,)
+        float32 tensor, valid where the last step's done is 1 (padding rows NaN)"""
+        rows = self._gather_rows(lambda b: b._episode_info, len(EPISODE_INFO_KEYS))
+        return OrderedDict((k, rows[:, j]) for j, k in enumerate(EPISODE_INFO_KEYS))
+
+    def step_infos(self):
+        """BatchedFurnitureEnv.step_infos of every bucket in global env order, num_envs dicts; padding rows are empty dicts"""
+        out = []
+        for b in self.buckets:
+            out.extend(b.step_infos())
+        return tuple(out) + ({},) * (self.num_envs - self.real_envs)
+
     def terminal_state(self):
         """BatchedFurnitureEnv.terminal_state of every bucket, in bucket order (bucket i holds the envs from offsets[i] on): the models' nq and nv
         differ, so the states are not stacked"""
@@ -641,12 +732,13 @@ class ShardedFurnitureEnv:
 
     `gather_info` widens the message by each env's info row (and, on a dense-reward shard, its dense_info row), so that step returns the
     info of every env and dense_infos() the dense rows of every env; `gather_terminal` widens it by the terminal observation, which
-    terminal_observation() returns for every env.  The step kernel writes the wider rows itself (Engine.set_packed_layout); a shard
-    without that kernel (MixedFurnitureEnv, a stand-in) has the same columns filled from its own step, terminal_observation() and
-    dense_infos()."""
+    terminal_observation() returns for every env; `gather_step_info` widens it by the reward terms and the episode record, which
+    reward_terms() and episode_record() return for every env.  The step kernel writes the wider rows itself (Engine.set_packed_layout,
+    Engine.set_packed_step_info); a shard without that kernel (MixedFurnitureEnv, a stand-in) has the same columns filled from its own
+    step, terminal_observation(), dense_infos(), reward_terms() and episode_record()."""
 
     def __init__(self, envs_per_gpu, agent="Sawyer", furniture_name="table_lack_0825", env=None, gather_info=False, gather_terminal=False,
-                 **cfg_overrides):
+                 gather_step_info=False, **cfg_overrides):
         import torch
         import torch.distributed as dist
 
@@ -661,10 +753,12 @@ class ShardedFurnitureEnv:
         self.gather_info, self.gather_terminal = bool(gather_info), bool(gather_terminal)
         layout = dict(info=self.gather_info, dense_info=self.gather_info and getattr(self.env, "dense_cfg", None) is not None,
                       terminal_obs=self.gather_terminal)
-        self._cols = packed_columns(self.env.obs_dim, **layout)
+        self.gather_step_info = bool(gather_step_info)
+        self._cols = packed_columns(self.env.obs_dim, step_info=self.gather_step_info, **layout)
         self._kernel = hasattr(self.env, "_stream")  # a BatchedFurnitureEnv: its step kernel writes the rows
         if self._kernel:
             self.env.engine.set_packed_layout(**layout)
+            self.env.engine.set_packed_step_info(self.gather_step_info)
         self.pack_dim = next(reversed(self._cols.values())).stop
         self._pack = torch.empty((envs_per_gpu, self.pack_dim), dtype=torch.float32, device=self.env.device)
         self._all = torch.empty((self.num_envs, self.pack_dim), dtype=torch.float32, device=self.env.device)
@@ -700,6 +794,12 @@ class ShardedFurnitureEnv:
             p[:, c["dense_info"]] = env.dense_infos()
         if "terminal_obs" in c:
             p[:, c["terminal_obs"]] = self.torch.cat(list(env.terminal_observation().values()), 1)
+        if "reward_info" in c:  # the terms (NaN on a dense shard, as the kernel writes them); the episode record where done, as in episode_info
+            t = self.torch
+            dense = getattr(env, "dense_cfg", None) is not None
+            p[:, c["reward_info"]] = float("nan") if dense else t.stack(list(env.reward_terms().values()), 1)
+            d = t.as_tensor(done, device=p.device).bool().reshape(-1, 1)
+            p[:, c["episode_info"]] = t.where(d, t.stack(list(env.episode_record().values()), 1).to(p.device), p[:, c["episode_info"]])
         return info
 
     def step(self, local_actions):
@@ -746,6 +846,20 @@ class ShardedFurnitureEnv:
         if "dense_info" not in self._cols:
             raise ValueError("dense_infos() needs ShardedFurnitureEnv(..., gather_info=True) on a shard that runs the dense reward")
         return self._all[:, self._cols["dense_info"]]
+
+    def reward_terms(self):
+        """{success_reward, touch_reward, pick_reward, ctrl_penalty} of every env after the last gathered step (gather_step_info=True), each a
+        (num_envs,) view of the message; NaN on a dense-reward shard, which has no such terms"""
+        if "reward_info" not in self._cols:
+            raise ValueError("reward_terms() needs ShardedFurnitureEnv(..., gather_step_info=True)")
+        return OrderedDict((k, self._all[:, self._cols["reward_info"].start + j]) for j, k in enumerate(REWARD_INFO_KEYS))
+
+    def episode_record(self):
+        """{episode_reward, episode_unstable} of every env (gather_step_info=True), each a (num_envs,) view of the last gathered message;
+        valid where its done is 1"""
+        if "episode_info" not in self._cols:
+            raise ValueError("episode_record() needs ShardedFurnitureEnv(..., gather_step_info=True)")
+        return OrderedDict((k, self._all[:, self._cols["episode_info"].start + j]) for j, k in enumerate(EPISODE_INFO_KEYS))
 
     def local_slice(self, gathered):
         """rows of this rank's own shard in a gathered (num_envs, ...) tensor"""

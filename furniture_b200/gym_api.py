@@ -17,7 +17,10 @@ on the keyword `terminal_observation`:
     `get_env_state()` gives the terminal state until the caller's `reset()`.  The step kernel writes both before its
     auto-reset; after an unstable step they are those of the reset inside `_do_simulation`'s except branch
     (furniture.py:2889-2897), as in the reference.
-`info` carries the reference's episode keys at the end of an episode (`_after_step`, furniture.py:451-480).
+`info` carries the reference's episode keys at the end of an episode (`_after_step`, furniture.py:451-480).  With the keyword
+`step_info=True` it is the reference's whole `info` dict: the sparse env adds `_compute_reward`'s four terms on every step
+(furniture.py:535-540), the two-arm env adds `ac` (furniture_baxter.py:75), `episode_reward` and `episode_unstable` come from the
+record the step kernel keeps, and a successful episode adds `episode_success_state`.  The default keeps the info described above.
 """
 from __future__ import annotations
 
@@ -30,11 +33,12 @@ import numpy as np
 class FurnitureGymB200:
     metadata = {"render.modes": []}
 
-    def __init__(self, name="FurnitureSawyerEnv", furniture_name=None, device=0, lib_path=None, id=None, terminal_observation=False, **config):
+    def __init__(self, name="FurnitureSawyerEnv", furniture_name=None, device=0, lib_path=None, id=None, terminal_observation=False,
+                 step_info=False, **config):
         """`id`, `name` and the remaining keywords are what gym passes from the registration (env/__init__.py:19-114: id, name,
         furniture_name / furniture_id, background, port ...); options of the renderer are ignored, see env.split_config.
         `terminal_observation`: step returns the terminal observation with done=True, as the reference's FurnitureEnv.step does (see the
-        module's docstring)"""
+        module's docstring).  `step_info`: step returns the reference's whole info dict (see the module's docstring)"""
         from .env import ENV_IDS, build_engine, env_options
 
         ids = dict(ENV_IDS, Sawyer=ENV_IDS["FurnitureSawyerEnv"], Baxter=ENV_IDS["FurnitureBaxterEnv"])  # and the bare agent names
@@ -53,6 +57,7 @@ class FurnitureGymB200:
         self._max_episode_steps = self.cfg.max_episode_steps
         self._pending_ob = None  # observation of an episode the device has already started
         self._terminal = bool(terminal_observation)
+        self._step_info = bool(step_info)
         self._terminal_state = None  # with terminal_observation: the state the finished episode ended in, until reset()
         self._episode_reward = 0.0
         self._episode_time = time.time()
@@ -108,6 +113,12 @@ class FurnitureGymB200:
 
             row = self.engine.get("dense_info")[0]
             out.update((k, float(v)) for k, v in zip(INFO_KEYS, row))
+        elif self._step_info:  # _compute_reward's terms (furniture.py:535-540), as the step kernel wrote them
+            from .engine import REWARD_INFO_KEYS
+
+            out.update((k, float(v)) for k, v in zip(REWARD_INFO_KEYS, self.engine.reward_info()[0]))
+        if self._step_info and self.engine.scene.narms == 2:
+            out["ac"] = a[0].copy()  # FurnitureBaxterEnv._step (furniture_baxter.py:75)
         if done:
             unstable = int(info[0][2])
             out["episode_success"] = int(info[0][1])
@@ -116,6 +127,12 @@ class FurnitureGymB200:
             out["episode_time"] = time.time() - self._episode_time
             out["episode_unstable"] = -float(self.cfg.unstable_penalty_coef) if unstable else 0
             out["episode_num_connected"] = int(info[0][0])
+            if self._step_info:  # the record the step kernel kept (float32 sum of the episode's rewards, plus the penalty)
+                rec = self.engine.episode_info()[0]
+                out["episode_reward"], out["episode_unstable"] = float(rec[0]), float(rec[1])
+                if out["episode_success"]:
+                    q, v = self.engine.terminal_state()
+                    out["episode_success_state"] = {"qpos": q[0].astype(np.float64), "qvel": v[0].astype(np.float64)}
             self._pending_ob = ob
             if self._terminal:  # the row and the state the step kernel kept before its auto-reset
                 ob = self._ob(self.engine.terminal_obs()[0])

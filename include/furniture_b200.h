@@ -22,6 +22,8 @@
  *                       tracked per env inside the kernels    furniture.py:103-107, :215-252, :1344-1387, :2723-2759
  *   fe_terminal_obs_dev / fe_terminal_qpos_dev / fe_terminal_qvel_dev <- the terminal `ob` of FurnitureEnv.step and the state
  *                       get_env_state gives at that point     furniture.py:364-385, :1781-1792
+ *   fe_reward_info_dev / fe_episode_info_dev <- the `info` dict of FurnitureEnv.step: _compute_reward's four terms and
+ *                       _after_step's episode record           furniture.py:451-541, :543-550
  *
  * Conventions: every function returns 0 on success or a negative code and records a message retrievable with
  * fe_last_error(); a handle is bound to one CUDA device, is not thread-safe, and all work is issued on the stream
@@ -216,12 +218,18 @@ int fe_env_step(fe_handle* h, const float* actions_dev, float* obs_dev, float* r
                    exactly (read them through an int32 view)                                 -- with fe_set_packed_layout's info = 1
      dense_info    fe_dense_info_dim() floats, the step's row of field "dense_info"          -- with dense_info = 1
      terminal_obs  obs_dim floats, the row the step also writes to terminal_obs              -- with terminal_obs = 1
-   The terminal slot of a row is valid where that step's done is 1 and is left untouched otherwise, exactly like terminal_obs.  With the
-   default layout the rows are [obs | reward | done], obs_dim + 2 floats, and nothing past them is written. */
+     step_info     6 floats: the step's row of field "reward_info" (NaN on a dense handle, which has no such row), then the 2 floats
+                   it writes to "episode_info"                                              -- with fe_set_packed_step_info's step_info = 1
+   The terminal slot and the last 2 floats of the step_info slot are valid where that step's done is 1 and are left untouched otherwise,
+   exactly like terminal_obs and episode_info.  With the default layout the rows are [obs | reward | done], obs_dim + 2 floats, and
+   nothing past them is written. */
 int fe_env_step_packed(fe_handle* h, const float* actions_dev, float* packed_dev, int32_t* info_dev, void* stream);
 /* What fe_env_step_packed writes after [obs | reward | done]: each flag 0 or 1, in effect from the next packed step.  Refused for a flag
    outside {0, 1}, for dense_info on a handle without the dense reward, and for a handle created without a scene blob. */
 int fe_set_packed_layout(fe_handle* h, int info, int dense_info, int terminal_obs);
+/* Whether fe_env_step_packed writes the step_info slot after the blocks of fe_set_packed_layout: 0 or 1, in effect from the next packed
+   step.  Refused for a value outside {0, 1} and for a handle created without a scene blob. */
+int fe_set_packed_step_info(fe_handle* h, int step_info);
 /* floats per packed row under the handle's layout at its current obs_dim (it follows fe_set_obs_layout): obs_dim + 2 by default */
 int fe_packed_dim(const fe_handle* h);
 /* same call with host buffers: H2D of the actions and D2H of the results happen inside (pinned staging) */
@@ -259,6 +267,22 @@ const float* fe_obs_dev(const fe_handle* h);
 const float* fe_terminal_obs_dev(const fe_handle* h);
 const float* fe_terminal_qpos_dev(const fe_handle* h);
 const float* fe_terminal_qvel_dev(const fe_handle* h);
+/* The step's info dict of the reference (FurnitureEnv._compute_reward / _after_step, furniture.py:451-541), written by every env step
+ * (fe_env_step, fe_env_step_packed, fe_env_step_host, under every control type):
+ *   reward_info   (n_envs, 4) float32, on every step of a sparse-reward handle: success_reward, touch_reward, pick_reward, ctrl_penalty,
+ *                 the terms the reward is made of (ctrl_penalty = -ctrl_penalty_coef * |a|^2, furniture.py:543-550).  On a step that is not
+ *                 unstable ((success_reward + touch_reward) + pick_reward) + ctrl_penalty is the step's reward; on an unstable step the
+ *                 reward adds the episode_unstable penalty.  A dense handle (fe_enable_dense_reward) has no such terms (they are
+ *                 dense_info): its steps write no row, the field stays NaN and fe_reward_info_dev returns NULL.
+ *   episode_info  (n_envs, 2) float32: episode_reward, episode_unstable of the episode the step ended -- the float32 sum of the episode's
+ *                 rewards before the penalty, plus the penalty, and the penalty (-unstable_penalty_coef after an unstable step, else 0).
+ *                 An unstable step resets the env inside the step first, as _do_simulation's except branch does (furniture.py:2889-2897),
+ *                 so its episode reports that step's reward alone, with length 1, like the reference's.
+ * A row of episode_info is valid where the last step's done is 1; the rows of the other envs are left as they are.  Rows no step has
+ * written hold NaN.  The same arrays are the read-only fields "reward_info" and "episode_info"; a handle created without a scene blob has
+ * neither the fields nor the buffers, and the accessors return NULL.  episode_time is a host clock and not part of the record. */
+const float* fe_reward_info_dev(const fe_handle* h);
+const float* fe_episode_info_dev(const fe_handle* h);
 
 /* ---- test hook: the device _is_aligned on explicit site poses (float64), n independent cases */
 int fe_is_aligned(fe_handle* h, int n, const double* p1, const double* m1, const double* p2, const double* m2, const double* angles /* (n,4) */,
